@@ -7,6 +7,7 @@ COMM_ID_BYTES = 128        # FPL_COMM_ID_BYTES == sizeof(ncclUniqueId)
 MAX_ADAPTER_LEN = 1024
 MAX_ADAPTERS = 1024
 INLINE_EVENTS = 4
+TAIL_PAD = 16              # FPL_TAIL_PAD
 
 PASS_FILTER, FAIL_POLY_X, FAIL_OVERLAP, FAIL_N_BASE = 0, 4, 8, 12
 FAIL_LENGTH, FAIL_TOO_LONG, FAIL_QUALITY, FAIL_COMPLEXITY = 16, 17, 20, 24
@@ -30,6 +31,11 @@ def stats_words(cycles):
 
 def counter_words(n_adapters):
     return CNT_FIXED + int(n_adapters) * 2 * (MAX_ADAPTER_LEN + 1)
+
+
+def batch_bytes(n_bytes):
+    """FPL_BATCH_BYTES: how many bytes of each buffer of a device batch of n_bytes the kernels may read"""
+    return (int(n_bytes) + 15) // 16 * 16 + TAIL_PAD
 
 
 def event_unpack(e):

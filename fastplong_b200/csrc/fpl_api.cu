@@ -73,7 +73,7 @@ struct fpl_ctx {
     bool emit_valid = false;            // the last call was a successful fpl_process_fastq_host: chunk + records + results in HBM
     int64_t emit_n = 0;
     int64_t last_bytes = 0;
-    bool slots16 = false;               // this batch's read offsets are multiples of 16 (checked: host batches, device ingest)
+    bool slots16 = false;               // this batch's read offsets are multiples of 16 (checked: host and device batches)
     int n_adapters = 0;
     uint8_t* d_adapters = nullptr;
     int* d_alen = nullptr;
@@ -524,17 +524,9 @@ int fpl_process_device(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results_
     const int64_t n = b->n_reads;
     if (n < 0) return fail("fpl_process_device: negative n_reads");
     DevBatch d = {b->seq, b->qual, b->offsets, b->lens, n};
-    if (c->tile_bases < (1ll << 61)) {       // read tiling was asked for: the tile boundaries need every length
-        c->h_lens.resize((size_t)n);
-        if (n) {
-            CK(cudaMemcpyAsync(c->h_lens.data(), b->lens, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, c->stream));
-            CK(cudaStreamSynchronize(c->stream));
-        }
-        c->slots16 = false;     // offsets not inspected on this path: the per-segment alignment dispatch handles anything
-        return run_batch(c, d, c->h_lens.data(), results_dev, b->n_bytes);
-    }
-    // only the extremes of the lengths are needed on the host (Stats capacity, grid sizes): reduce them on the side
-    // stream, which does not wait for the kernels of the previous batch still running on the compute stream
+    // the extremes of the lengths (Stats capacity, grid sizes) and the alignment of the offsets are all the host needs
+    // to know: reduce them on the side stream, which does not wait for the kernels of the previous batch still running
+    // on the compute stream
     if (!c->copy_stream) CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
     if (!c->d_minmax) {
         CK(cudaMalloc(&c->d_minmax, 4 * sizeof(int)));
@@ -549,8 +541,17 @@ int fpl_process_device(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results_
         CK(cudaMemcpyAsync(c->h_minmax, c->d_minmax, 3 * sizeof(int), cudaMemcpyDeviceToHost, c->copy_stream));
         CK(cudaStreamSynchronize(c->copy_stream));
         if (c->h_minmax[0] < 0) return fail("fpl_process_device: a read has a negative length");
+        if (c->h_minmax[2]) return fail("fpl_process_device: a read offset is not a multiple of 16 (see fpl_batch)");
     }
-    c->slots16 = c->h_minmax[2] == 0;
+    c->slots16 = true;
+    if (c->tile_bases < (1ll << 61)) {       // read tiling was asked for: the tile boundaries need every length
+        c->h_lens.resize((size_t)n);
+        if (n) {
+            CK(cudaMemcpyAsync(c->h_lens.data(), b->lens, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, c->stream));
+            CK(cudaStreamSynchronize(c->stream));
+        }
+        return run_batch(c, d, c->h_lens.data(), results_dev, b->n_bytes);
+    }
     return run_batch(c, d, nullptr, results_dev, b->n_bytes, nullptr, nullptr, n ? c->h_minmax[1] : 0);
 }
 
@@ -580,7 +581,7 @@ int fpl_process_host(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results) {
             return fail("fpl_process_host: read %lld has a bad slot (offset %lld, len %d, n_bytes %lld; offsets must be multiples of 16)",
                         (long long)i, (long long)o, b->lens[i], (long long)b->n_bytes);
     }
-    const int64_t need = b->n_bytes + 64;  // tail pad for whole-word over-reads
+    const int64_t need = FPL_BATCH_BYTES(b->n_bytes);  // the tail the kernels' whole-vector reads may touch
     if (need > c->cap_bytes) {
         cudaFree(c->d_seq); cudaFree(c->d_qual); c->d_seq = c->d_qual = nullptr; c->cap_bytes = 0;
         CK(cudaMalloc(&c->d_seq, need));
@@ -622,8 +623,8 @@ int fpl_process_host(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results) {
             CK(cudaMemcpyAsync(c->d_qual + lo, b->qual + lo, hi - lo, cudaMemcpyHostToDevice, cs));
         }
         if (j + 1 == np) {
-            CK(cudaMemsetAsync(c->d_seq + b->n_bytes, 0, 64, cs));
-            CK(cudaMemsetAsync(c->d_qual + b->n_bytes, 0, 64, cs));
+            CK(cudaMemsetAsync(c->d_seq + b->n_bytes, 0, need - b->n_bytes, cs));
+            CK(cudaMemsetAsync(c->d_qual + b->n_bytes, 0, need - b->n_bytes, cs));
         }
         CK(cudaEventRecord(c->piece_events[j], cs));
     }
@@ -653,7 +654,7 @@ int fpl_process_fastq_host(fpl_ctx* c, const uint8_t* text, int64_t n_bytes, int
     if (nrec > max_records) return 1;
     if (!records || !results) return fail("fpl_process_fastq_host: records/results is null");
     FplIngest& g = c->ingest;
-    const int64_t need = g.packed_bytes + 64;
+    const int64_t need = FPL_BATCH_BYTES(g.packed_bytes);
     if (need > c->cap_bytes) {
         cudaFree(c->d_seq); cudaFree(c->d_qual); c->d_seq = c->d_qual = nullptr; c->cap_bytes = 0;
         CK(cudaMalloc(&c->d_seq, need));

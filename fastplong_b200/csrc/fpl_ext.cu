@@ -317,8 +317,10 @@ int fpl_ext_run(FplExt* x, const DevParams& P, const DevBatch& b, int64_t n_byte
     if (growb((void**)&x->d_stat, &x->cap_stat, (int64_t)sizeof(StatSeg) * (total + 1), err, errlen)) return -1;
     k_ext_emit<<<g2, 256, 0, s>>>(P, b, res, x->d_off, x->d_segs);
     if (P.opt.mask_enabled && total > 0) {
-        if (growb((void**)&x->d_mseq, &x->cap_mseq, n_bytes + 64, err, errlen)) return -1;
+        // the masked copy is a batch of its own: its tail pad is defined, not whatever the buffer held before
+        if (growb((void**)&x->d_mseq, &x->cap_mseq, FPL_BATCH_BYTES(n_bytes), err, errlen)) return -1;
         CKE(cudaMemcpyAsync(x->d_mseq, b.seq, (size_t)n_bytes, cudaMemcpyDeviceToDevice, s));
+        CKE(cudaMemsetAsync(x->d_mseq + n_bytes, 0, (size_t)(FPL_BATCH_BYTES(n_bytes) - n_bytes), s));
         if (growb((void**)&x->d_rcnt, &x->cap_rcnt, (int64_t)sizeof(int32_t) * (total + 1), err, errlen)) return -1;
         if (growb((void**)&x->d_roff, &x->cap_roff, (int64_t)sizeof(int32_t) * (total + 1), err, errlen)) return -1;
         const unsigned gs = (unsigned)((total + 255) / 256);

@@ -106,9 +106,17 @@ typedef struct fpl_adapters {
 /*
  * A packed batch of reads: sequence bytes and quality bytes in two buffers with identical layout;
  * read i occupies [offsets[i], offsets[i]+lens[i]) in both.  Offsets must be multiples of 16 and the
- * buffers 16-byte aligned (vector loads / TMA bulk copies); bytes between slots are ignored.
+ * buffers 16-byte aligned (vector loads / TMA bulk copies); fpl_process_host and fpl_process_device both
+ * reject an offset that is not a multiple of 16.  Slots may lie in any order, with any gaps; the bytes
+ * between and behind them are ignored, whatever they hold.
+ * The kernels load whole 16- and 32-byte vectors from 16-byte boundaries, so they may read up to
+ * FPL_TAIL_PAD bytes behind the 16-byte vector that holds byte n_bytes - 1, and nothing in front of
+ * offset 0: a DEVICE batch's two buffers must each be readable for FPL_BATCH_BYTES(n_bytes) bytes.  A host
+ * batch needs no such pad (fpl_process_host adds it on the device).
  * Replaces ReadPack{Read** data; int count} (src/read.h:63-66) — many 16-read packs per submission.
  */
+#define FPL_TAIL_PAD 16
+#define FPL_BATCH_BYTES(n_bytes) ((((int64_t)(n_bytes) + 15) & ~(int64_t)15) + FPL_TAIL_PAD)
 typedef struct fpl_batch {
     const uint8_t* seq;
     const uint8_t* qual;
@@ -241,9 +249,11 @@ void fpl_destroy(fpl_ctx* ctx);
 int fpl_process_host(fpl_ctx* ctx, const fpl_batch* host_batch, fpl_read_result* results);
 
 /*
- * Same, for a batch already resident in DEVICE memory (all four pointers are device pointers);
+ * Same, for a batch already resident in DEVICE memory (all four pointers are device pointers; seq and qual
+ * readable for FPL_BATCH_BYTES(n_bytes) bytes, see fpl_batch);
  * results_dev is a device array of n_reads records or NULL to keep results in the context's own buffer.
- * Asynchronous on the context's stream; fpl_sync() waits.
+ * Checks the offsets' alignment and the lengths' signs on the device first (an error if any fails), then
+ * runs asynchronously on the context's stream; fpl_sync() waits.
  */
 int fpl_process_device(fpl_ctx* ctx, const fpl_batch* dev_batch, fpl_read_result* results_dev);
 int fpl_sync(fpl_ctx* ctx);

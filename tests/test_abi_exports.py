@@ -37,6 +37,12 @@ def test_struct_mirror_sizes():
     assert int(re.search(r"#define FPL_MAX_ADAPTER_LEN (\d+)", hdr).group(1)) == abi.MAX_ADAPTER_LEN
     assert int(re.search(r"#define FPL_STATS_TAIL (\d+)", hdr).group(1)) == abi.STATS_TAIL
     assert int(re.search(r"#define FPL_CNT_FIXED (\d+)", hdr).group(1)) == abi.CNT_FIXED
+    assert int(re.search(r"#define FPL_TAIL_PAD (\d+)", hdr).group(1)) == abi.TAIL_PAD
+    # FPL_BATCH_BYTES(n) evaluated from its text (the int64_t casts dropped; every n here is >= 0) against abi.batch_bytes
+    body = re.search(r"#define FPL_BATCH_BYTES\(n_bytes\) (.*)", hdr).group(1).replace("(int64_t)", "")
+    for n in (0, 1, 15, 16, 17, 31, 32, 33, 149, 4097, 123456789):
+        assert eval(body.replace("FPL_TAIL_PAD", str(abi.TAIL_PAD)), {"n_bytes": n}) == abi.batch_bytes(n), n
+    assert [abi.batch_bytes(n) for n in (0, 1, 16, 17)] == [16, 32, 32, 48]
 
 
 @pytest.mark.skipif(not os.path.exists(binding.LIB_PATH), reason="libfplgpu.so not built")
