@@ -109,6 +109,10 @@ typedef struct fpl_adapters {
  * buffers 16-byte aligned (vector loads / TMA bulk copies); fpl_process_host and fpl_process_device both
  * reject an offset that is not a multiple of 16.  Slots may lie in any order, with any gaps; the bytes
  * between and behind them are ignored, whatever they hold.
+ * Every sequence and quality byte INSIDE a read must be below 0x80 (the reference indexes 128-entry
+ * tables with them).  This is not checked: the kernels pack several quality bytes into one word and read
+ * bit 7 of each as a flag, so a byte >= 0x80 gives wrong counts and Stats, not an error.  Quality bytes
+ * below '!' (33) are valid and count as negative qualities, as in the reference.
  * The kernels load whole 16- and 32-byte vectors from 16-byte boundaries, so they may read up to
  * FPL_TAIL_PAD bytes behind the 16-byte vector that holds byte n_bytes - 1, and nothing in front of
  * offset 0: a DEVICE batch's two buffers must each be readable for FPL_BATCH_BYTES(n_bytes) bytes.  A host

@@ -304,7 +304,90 @@ def _extreme_sets():
         "qual_phred0_limits0": Options(start_adapter=S, qualified_quality_phred=0, unqualified_percent_limit=0, n_base_limit=0, n_percent_limit=0),
         "mask_break_w5_q30": Options(start_adapter=S, mask=True, mask_window_size=5, mask_mean_quality=30, break_reads=True,
                                      break_window_size=5, break_mean_quality=30),
+        **QUALITY_SETS,
     }
+
+
+# ---- the whole quality-byte range: bytes 1..127 (a 0 byte cannot reach the reference, which builds its reads from C strings)
+# and the quality options at the ends of what src/options.cpp:validate accepts: -q 0..93, --mean_qual 0..93, the cut
+# qualities 1..30 (the help text says 1~36; the validator is what holds).  validate does not check the --mask / --break
+# qualities at all (the help text says 5~30): they run here at 1 and 93, the ends of the phred range a 7-bit byte can reach.
+QUALITY_SETS = {
+    "q93": Options(start_adapter=S, qualified_quality_phred=93, unqualified_percent_limit=60),
+    "q0": Options(start_adapter=S, end_adapter=E, qualified_quality_phred=0, unqualified_percent_limit=0),
+    "mean_qual93": Options(start_adapter=S, mean_qual=93, unqualified_percent_limit=100),
+    "mean_qual1": Options(start_adapter=S, mean_qual=1, low_complexity_filter=True),
+    "cut_q1_w4": Options(start_adapter=S, cut_front=True, cut_tail=True, cut_window_size=4, cut_mean_quality=1),
+    "cut_q30_w1": Options(disable_adapter_trimming=True, cut_front=True, cut_tail=True, cut_window_size=1, cut_mean_quality=30,
+                          length_required=1),
+    "cut_front_q1_tail_q30": Options(start_adapter=S, end_adapter=E, cut_front=True, cut_tail=True, cut_front_window_size=10,
+                                     cut_front_mean_quality=1, cut_tail_window_size=5, cut_tail_mean_quality=30),
+    "mask_q1_break_q93": Options(start_adapter=S, mask=True, mask_window_size=5, mask_mean_quality=1, break_reads=True,
+                                 break_window_size=10, break_mean_quality=93),
+    "mask_q93_break_q1": Options(start_adapter=S, mask=True, mask_window_size=10, mask_mean_quality=93, break_reads=True,
+                                 break_window_size=5, break_mean_quality=1),
+    "mask_q20_w4": Options(start_adapter=S, mask=True, mask_window_size=4, mask_mean_quality=20, length_required=1),
+}
+
+
+def _window_on(rng, w, total):
+    """w quality bytes in 1..127 whose sum is exactly `total` (w <= total <= 127 * w), some of them below 33"""
+    q = rng.integers(1, 128, size=w)
+    while q.sum() != total:
+        i = int(rng.integers(w))
+        step = int(np.sign(total - q.sum()))
+        if 1 <= q[i] + step <= 127:
+            q[i] += step
+    return bytes(q.astype(np.uint8))
+
+
+def quality_domain_batch(seed, n_random=60):
+    """Reads whose quality bytes cover 1..127: long runs below 33 ('!' is 33), runs of 127, reads whose qualities are all below
+    33 (a negative totalQual, Stats' quality sums going down), windows whose raw byte sum is exactly (33 + M) * w of a cut /
+    mask / break window (and one more and one less) for the M and w of QUALITY_SETS and the defaults, and reads of bytes drawn
+    uniformly from 1..127.  Start / end adapters and N now and then."""
+    rng = np.random.default_rng(seed)
+    reads = []
+
+    def seq(n):
+        s = bytearray(_rb(rng, n))
+        for p in rng.integers(0, n, size=n // 200):
+            s[int(p)] = ord("N")
+        if n > 120 and rng.random() < 0.4:
+            s[:30] = S.encode()
+        if n > 120 and rng.random() < 0.3:
+            s[n - 30:] = E.encode()
+        return bytes(s)
+
+    def uniform(n, lo=1, hi=127):
+        return bytes(rng.integers(lo, hi + 1, size=n).astype(np.uint8))
+
+    for k in range(12):                                           # runs below 33 and runs of 127 inside ordinary reads
+        n = int(rng.integers(200, 1500))
+        q = bytearray(uniform(n, 33 + 5, 33 + 40))
+        for _ in range(3):
+            a, m = int(rng.integers(0, n)), int(rng.integers(20, 300))
+            q[a:a + m] = uniform(len(q[a:a + m]), 1, 32) if k % 2 else b"\x7f" * len(q[a:a + m])
+        reads.append((seq(n), bytes(q)))
+    for n in (1, 2, 5, 31, 32, 33, 100, 700):                     # every byte below 33: totalQual < 0
+        reads.append((seq(n), uniform(n, 1, 32)))
+        reads.append((seq(n), b"\x01" * n))
+        reads.append((seq(n), b"\x7f" * n))
+    for M in (1, 10, 15, 20, 30, 93):                             # windows exactly on the threshold, one above, one below
+        for w in (1, 4, 5, 10):
+            for d in (-1, 0, 1):
+                total = (33 + M) * w + d
+                if not w <= total <= 127 * w:
+                    continue
+                win = _window_on(rng, w, total)
+                low, good = uniform(40, 1, 20), uniform(60, 33 + M, 127)
+                reads.append((seq(100 + w), low + win + good))                # a front cut starts here or not
+                reads.append((seq(100 + w), good + win + low))                # a tail cut ends here or not
+                reads.append((seq(100 + 3 * w), good[:50] + win * 3 + good[:50]))   # mask / break windows in the middle
+    for _ in range(n_random):
+        n = int(rng.integers(50, 2000))
+        reads.append((seq(n), uniform(n)))
+    return pack_reads(reads)
 
 
 EXTREME_SETS = _extreme_sets()
@@ -323,6 +406,11 @@ MASK_BREAK_SETS = {
     "break_no_adapter": Options(disable_adapter_trimming=True, break_reads=True, break_window_size=25,
                                 break_mean_quality=12, disable_quality_filtering=True),
 }
+
+# the option sets that run on quality_domain_batch: QUALITY_SETS and sets of every other kind (adapters with the complexity
+# filter, the global trims with --mean_qual, a one-base tail window, --mask with --break and the cuts)
+QUALITY_DOMAIN_SETS = dict(QUALITY_SETS, **{n: OPTION_SETS[n] for n in ("default_se", "cut_polyx_cplx", "trims_limits", "loose_ed")},
+                           mask_and_break=MASK_BREAK_SETS["mask_and_break"])
 
 
 def blocky_quality_batch(seed, n=150):

@@ -226,6 +226,77 @@ def load_jit(amax=30):
     return lib
 
 
+# ---- the byte-packed quality step of the whole-read scans: k_scan_jit v2 (x = q + KQ, unsigned and signed dp4a) and
+# k_scan_fast ((q | 0x80) - Q per byte), the kernels' own lines ----
+QUAL_HARNESS = r"""
+extern "C" {
+// k_scan_jit v2 over n quality words at qualified char FPL_QQ: #(q >= qualified) and sum(q - 33) as the kernel derives them
+void j_qual_words(const uint32_t* q, int n, int FPL_QQ, int* ge_out, int* sum_out) {
+    const uint32_t one = 1u;
+    @@KQ@@
+    uint32_t accU = 0;
+    int accS = 0;
+    for (int k = 0; k < n; k++) {
+        @@STEP@@
+    }
+    const int nbytes = 4 * n;
+    int ge = @@GE@@;
+    int sumq = (int)accU;
+    *ge_out = ge;
+    *sum_out = @@SUM@@;
+}
+// k_scan_fast's word step over n words
+void f_qual_words(const uint32_t* words, int n, int qualified_qual, int* ge_out, int* sum_out) {
+    @@QQ4@@
+    int lowq_ge = 0, totalq = 0;
+    for (int k = 0; k < n; k++) {
+        const uint32_t q = words[k];
+        @@FSTEP@@
+    }
+    *ge_out = lowq_ge;
+    *sum_out = totalq - 33 * 4 * n;
+}
+}
+"""
+
+
+def _one(pattern, text, what):
+    m = re.search(pattern, text, re.S)
+    if not m:
+        raise KeyError(f"{what} not found")
+    return m.group(1)
+
+
+def qual_step_source():
+    raw = open(os.path.join(CSRC, "fpl_scan_jit2_src.h")).read()
+    fast = open(os.path.join(CSRC, "fpl_scan_fast.cu")).read()
+    kq = _one(r"constexpr (uint32_t KQ = \(uint32_t\)\(128 - \(FPL_QQ & 0x7f\)\);)", raw, "KQ of k_scan_jit")
+    step = _one(r"if \(interior\) \{\s*#pragma unroll\s*for \(int k = 0; k < 8; k\+\+\) \{\s*(const uint32_t x = mad_u32.*?accS\);)\s*\}", raw,
+                "the interior quality step of k_scan_jit")
+    ge = _one(r"int ge = (\(int\)\(\(accU - \(uint32_t\)accS\) >> 8\));", raw, "the count of k_scan_jit")
+    sm = _one(r"sh32\[2\]\[wid\] = (sumq - \(int\)\(KQ \+ 33u\) \* nbytes);", raw, "the quality sum of k_scan_jit")
+    qq4 = _one(r"(const uint32_t qq4 = \(uint32_t\)\(P\.opt\.qualified_qual & 0x7f\) \* 0x01010101u;)", fast, "qq4 of k_scan_fast")
+    fstep = _one(r"\n\s*(totalq = \(int\)__dp4a\(q, 0x01010101u, \(unsigned\)totalq\);\s*lowq_ge \+= __popc\([^;]*;)", fast,
+                 "the word step of k_scan_fast")
+    h = (QUAL_HARNESS.replace("@@KQ@@", "const " + kq).replace("@@STEP@@", step).replace("@@GE@@", ge).replace("@@SUM@@", sm)
+         .replace("@@QQ4@@", qq4.replace("P.opt.qualified_qual", "qualified_qual")).replace("@@FSTEP@@", fstep))
+    return "\n".join([SHIMS, "static inline int __popc(uint32_t x) { return __builtin_popcount(x); }",
+                      _asm_to_c(extract(os.path.join(CSRC, "fpl_stats.cu"), "mad_u32", "func")), h])
+
+
+def load_qual_step():
+    src = qual_step_source()
+    so = f"/tmp/fpl_qual_step_{hashlib.md5(src.encode()).hexdigest()[:12]}.so"
+    if not os.path.exists(so):
+        cpp = so[:-3] + ".cpp"
+        open(cpp, "w").write(src)
+        subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", "-I", os.path.join(ROOT, "include"), "-o", so, cpp])
+    lib = C.CDLL(so)
+    for f in (lib.j_qual_words, lib.f_qual_words):
+        f.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    return lib
+
+
 _lib = None
 
 

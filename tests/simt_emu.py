@@ -193,12 +193,16 @@ def emulated_library():
 
 
 class _Bound:
-    """binding's module state pointed at the emulated library for the duration of a `with` block"""
+    """binding's module state pointed at the emulated library (or at `lib`, another emulated build) for the duration of a
+    `with` block"""
+
+    def __init__(self, lib=None):
+        self.lib = lib
 
     def __enter__(self):
         from fastplong_b200 import binding
         self.binding, self.saved = binding, (binding.LIB_PATH, binding._lib)
-        path = build_library()
+        path = self.lib or build_library()
         binding.LIB_PATH, binding._lib = path, _Bound.libs.get(path)
         _Bound.libs[path] = binding.load_library()
         return binding
@@ -210,17 +214,17 @@ class _Bound:
 _Bound.libs = {}      # path -> loaded handle (a mutant build is another path)
 
 
-def EmuEngine(options, scan="jit"):
+def EmuEngine(options, scan="jit", lib=None):
     """binding.Engine(options) on the emulated library.  scan: which whole-read scan kernel fpl_create sets up — "jit": the default
     (k_scan_jit specialised through the NVRTC stand-in wherever the library specialises), "fast": FPL_NO_JIT=1 (the precompiled
-    k_scan_fast), "generic": FPL_FORCE_GENERIC_SCAN=1 (k_scan)."""
+    k_scan_fast), "generic": FPL_FORCE_GENERIC_SCAN=1 (k_scan).  lib: the path of another emulated build (build_library(override))."""
     env = {"jit": {}, "fast": {"FPL_NO_JIT": "1"}, "generic": {"FPL_FORCE_GENERIC_SCAN": "1"}}[scan]
     saved = {k: os.environ.get(k) for k in ("FPL_NO_JIT", "FPL_FORCE_GENERIC_SCAN")}
     for k in saved:
         os.environ.pop(k, None)
     os.environ.update(env)
     try:
-        with _Bound() as binding:
+        with _Bound(lib) as binding:
             return binding.Engine(options)
     finally:
         for k, v in saved.items():

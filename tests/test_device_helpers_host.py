@@ -290,3 +290,28 @@ def test_scan_bit_sliced_count_comparison_is_exact(amax):
             for i in range(32):
                 exp |= int(counts[i] >= g) << i
             assert lib.j_ge_mask(c.ctypes.data, row.ctypes.data) == exp, (case, g)
+
+
+@pytest.mark.parametrize("fn", ["j_qual_words", "f_qual_words"])
+def test_scan_quality_step_over_every_quality_byte(fn):
+    """The byte-packed quality counts of the whole-read scans, the kernels' own lines: k_scan_jit adds x = q + (128 - Q) per
+    byte with an unsigned and a signed dp4a ((accU - accS) >> 8 = #(q >= Q), accU - (KQ + 33) * n = sum(q - 33)); k_scan_fast
+    counts bit 7 of (q | 0x80) - Q per byte.  Every q in 0..127 in every byte lane, the other lanes random, for every
+    qualified char Q of -q 0..93 (33..126); then long runs of words at the extreme bytes, where the sums are largest."""
+    lib = device_helpers.load_qual_step()
+    f = getattr(lib, fn)
+    ge, sm = C.c_int(), C.c_int()
+    rng = np.random.default_rng(27)
+    for Q in range(33, 127):
+        for lane in range(4):
+            bs = rng.integers(0, 128, size=(128, 4)).astype(np.uint8)
+            bs[:, lane] = np.arange(128)
+            for row in bs:
+                w = np.ascontiguousarray(row).view("<u4").copy()
+                f(w.ctypes.data, 1, Q, C.byref(ge), C.byref(sm))
+                assert (ge.value, sm.value) == (int((row >= Q).sum()), int(row.astype(np.int64).sum()) - 33 * 4), (fn, Q, list(row))
+        for b in (0, 1, 32, 33, Q - 1, Q, 126, 127):
+            for n in (1, 8, 4096):
+                w = np.full(n, b * 0x01010101, dtype=np.uint32)
+                f(w.ctypes.data, n, Q, C.byref(ge), C.byref(sm))
+                assert (ge.value, sm.value) == (4 * n * int(b >= Q), 4 * n * (b - 33)), (fn, Q, b, n)

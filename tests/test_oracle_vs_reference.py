@@ -85,6 +85,24 @@ def test_extreme_option_values(name):
     compare_stats(o.counters(), r.counters(), name + "/counters")
 
 
+@pytest.mark.parametrize("name", sorted(cases.QUALITY_DOMAIN_SETS))
+def test_quality_bytes_1_to_127(name):
+    """quality bytes over the whole range the reference takes (1..127: runs below '!', runs of 127, all-low reads whose
+    totalQual is negative, windows exactly on a cut / mask / break threshold) under -q 0 / 93, --mean_qual 1 / 93 and the cut,
+    mask and break qualities at the ends of what the CLI accepts"""
+    opt = cases.QUALITY_DOMAIN_SETS[name]
+    batch = cases.quality_domain_batch(21)
+    o, r = OracleEngine(opt), RefEngine(opt)
+    compare_results(o.process(batch), r.process(batch), name)
+    if opt.mask or opt.break_reads:
+        compare_lists(o.segments(), r.segments(), name + "/segments")
+        compare_lists(o.mask_regions(), r.mask_regions(), name + "/regions")
+    cyc = int(batch.lens.max())
+    for w in (0, 1):
+        compare_stats(o.stats(w, cyc), r.stats(w, cyc), f"{name}/stats{w}")
+    compare_stats(o.counters(), r.counters(), name + "/counters")
+
+
 def test_empty_batch():
     check(cases.OPTION_SETS["default_se"], pack_reads([]), "empty")
 

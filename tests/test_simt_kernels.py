@@ -88,6 +88,14 @@ def test_extreme_option_values(name):
     check(cases.EXTREME_SETS[name], batch, name)
 
 
+@pytest.mark.parametrize("scan", ["jit", "fast", "generic"])
+@pytest.mark.parametrize("name", sorted(cases.QUALITY_DOMAIN_SETS))
+def test_quality_bytes_1_to_127(name, scan):
+    """cases.quality_domain_batch (bytes 1..127, pinned oracle-vs-reference) through each of the three whole-read scans, whose
+    quality counts are byte-packed: x = q + (128 - Q) with unsigned and signed dp4a (k_scan_jit), (q | 0x80) - Q (k_scan_fast)"""
+    check(cases.QUALITY_DOMAIN_SETS[name], cases.quality_domain_batch(21), f"{name}/{scan}", scan)
+
+
 @pytest.mark.parametrize("name", sorted(cases.RNA_SETS))
 @pytest.mark.parametrize("mixed", [False, True])
 def test_rna_reads(name, mixed):

@@ -94,3 +94,23 @@ def test_filter_counts_of_the_other_scan_kernels(name, switch, monkeypatch):
     monkeypatch.setenv(switch, "1")
     opt, batch = cases.edge_cases()[name]
     check_against_oracle(opt, batch, f"{name}/{switch}")
+
+
+def _quality_names():
+    import cases
+    return sorted(cases.QUALITY_DOMAIN_SETS)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("switch", [None, "FPL_NO_JIT", "FPL_FORCE_GENERIC_SCAN"])
+@pytest.mark.parametrize("name", _quality_names())
+def test_quality_bytes_1_to_127_vs_oracle(name, switch, monkeypatch):
+    """cases.quality_domain_batch (quality bytes 1..127, pinned oracle-vs-reference on the CPU) under the extreme quality
+    options, through k_scan_jit, k_scan_fast and the generic k_scan: records, both Stats blocks, counters, the -N/-b lists"""
+    import capacity
+    import cases
+    from fastplong_b200.binding import Engine
+    if switch:
+        monkeypatch.setenv(switch, "1")
+    opt = cases.QUALITY_DOMAIN_SETS[name]
+    capacity.compare_with_oracle(Engine(opt), opt, cases.quality_domain_batch(21), f"{name}/{switch}")

@@ -1,9 +1,11 @@
 """Development aid (CPU): mutation testing of the GPU tests' grip on the KERNELS.  A sample of single-token mutants of the kernel
 sources (comparison operators, && / ||, +-1) is built into the emulated library (tests/simt_emu.py) and run against the oracle on
-a battery — crafted boundaries, option matrix on adversarial reads, RNA, -N/-b, FASTQ text.  A surviving mutant is kernel
+a battery — crafted boundaries, option matrix on adversarial reads, RNA, -N/-b, FASTQ text, and the capacity limits of the
+statistics and text kernels (tests/test_capacity_shrunk.py's cases on the mutant built with shrunk constants, the packed
+counter of k_cycle_stats at its fullest).  A surviving mutant is kernel
 behaviour the parity tests do not pin — or an equivalent mutant: the one-sided filters (a filter that says "maybe" more often
 changes no result by design), min / max ties, guards that cannot fire.
-usage: python tools/mutate_kernels.py <file.cu> <n_mutants> [seed] [workers]      (internal: --battery <lib.so>)"""
+usage: python tools/mutate_kernels.py <file.cu> <n_mutants> [seed] [workers]      (internal: --battery <lib.so> [<shrunk lib.so>])"""
 import os
 import random
 import re
@@ -18,14 +20,29 @@ OPS = [(r"<=", "<"), (r">=", ">"), (r"(?<![<>=!-])<(?![<=])", "<="), (r"(?<![<>=
        (r"&&", "||"), (r"\|\|", "&&"), (r"\+ 1\b", "+ 0"), (r"- 1\b", "- 0")]
 
 
-def battery(lib):
+SHRUNK = "group_of_2_stages"       # tests/test_capacity_shrunk.py: the build whose capacities the battery's small cases reach
+
+
+def battery(lib, small=None):
     import signal
     import simt_emu
     simt_emu._emu_lib_path = lib
+    import capacity
     import cases
+    import test_capacity_shrunk as CS
     import test_simt_kernels as T
-    signal.alarm(600)
+    signal.alarm(900)
     try:
+        # the capacity limits: the mutant built with shrunk constants, and the packed counter at its fullest at full size
+        if small:
+            CS.LIBS[SHRUNK] = (small, capacity.constants(capacity.shrunk_sources(**CS.BUILDS[SHRUNK])))
+            for optset in sorted(capacity.CS_SETS):
+                CS.test_cycle_stats_staging_rounds_and_groups(SHRUNK, optset)
+                CS.test_cycle_stats_post_filter_counts(SHRUNK, optset)
+            CS.test_kmer_fix_long_range_list(SHRUNK)
+            CS.test_read_qual_long_list_and_stride(SHRUNK)
+            CS.test_text_path_more_records_than_warps(SHRUNK)
+        T.check(capacity.HEADROOM_OPT, capacity.headroom_batch(capacity.constants(), False), "packed counter at its fullest")
         for name, (opt, b) in cases.edge_cases().items():
             T.check(opt, b, name)
         adv = cases.adversarial_batch(1)
@@ -73,27 +90,31 @@ def candidates(text):
 
 
 def run_one(args):
+    import capacity
     import simt_emu
+    import test_capacity_shrunk
     k, fn, text, (li, a, b, rep) = args
     lines = text.split("\n")
     new = lines[li][:a] + rep + lines[li][b:]
     mutated = "\n".join(lines[:li] + [new] + lines[li + 1:])
     try:
         lib = simt_emu.build_library({fn: mutated})
+        small = simt_emu.build_library(capacity.shrunk_sources({fn: mutated}, **test_capacity_shrunk.BUILDS[SHRUNK]))
     except Exception:
         return k, "nocompile", lines[li], new
     try:
-        p = subprocess.run([sys.executable, os.path.abspath(__file__), "--battery", lib], capture_output=True, text=True, timeout=900)
+        p = subprocess.run([sys.executable, os.path.abspath(__file__), "--battery", lib, small], capture_output=True, text=True,
+                           timeout=1200)
         out = p.stdout.strip().split("\n")[-1] if p.stdout.strip() else "KILLED (crash)"
     except subprocess.TimeoutExpired:
         out = "KILLED (timeout)"
-    subprocess.run(["rm", "-rf", os.path.dirname(lib)])
+    subprocess.run(["rm", "-rf", os.path.dirname(lib), os.path.dirname(small)])
     return k, out, lines[li], new
 
 
 if __name__ == "__main__":
     if sys.argv[1] == "--battery":
-        battery(sys.argv[2])
+        battery(*sys.argv[2:4])
         sys.exit(0)
     fn, count = sys.argv[1], int(sys.argv[2])
     rng = random.Random(int(sys.argv[3]) if len(sys.argv) > 3 else 1)
