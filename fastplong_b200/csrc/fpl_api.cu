@@ -34,7 +34,7 @@ void launch_scan_fast(const DevParams&, const ScanPlan&, const DevBatch&, ReadSt
 void launch_final(const DevParams&, const DevBatch&, const ReadState*, fpl_read_result*, StatSeg*, cudaStream_t);
 void launch_count(const fpl_read_result*, int64_t, unsigned long long*, bool, cudaStream_t);
 int launch_cycle_stats(CycleWs*, const uint8_t*, const uint8_t*, const StatSeg*, int64_t, int64_t, unsigned long long*, int64_t,
-                        bool, unsigned long long*, bool, cudaStream_t);
+                        bool, unsigned long long*, bool, const StatSeg*, unsigned long long*, const StatSeg*, cudaStream_t);
 void launch_kmer_fix(const DevBatch&, const fpl_read_result*, unsigned long long*, cudaStream_t);
 void launch_read_qual(const DevBatch&, unsigned long long*, unsigned long long*, int64_t, fpl_read_result*, bool, cudaStream_t);
 void launch_make_preseg(const DevBatch&, StatSeg*, cudaStream_t);
@@ -56,9 +56,11 @@ static int fail(const char* fmt, ...) {
     } while (0)
 
 enum { K_PRESEG, K_CYCLE_PRE, K_QUAL_PRE, K_TRIM, K_SCAN, K_FINAL, K_COUNT, K_CYCLE_POST, K_QUAL_POST, K_KMER_FIX, K_ALLREDUCE, K_NKERNELS };
-static const char* const kKernelNames[K_NKERNELS] = {"k_make_preseg", "k_cycle_stats(pre)", "k_read_qual(pre+post)",
+// K_CYCLE_PRE: the fused pass (both Stats blocks) without --mask/--break, the pre-filter pass with it; K_CYCLE_POST: the
+// post-filter segments the fused pass did not take, or the whole --mask/--break post-filter list
+static const char* const kKernelNames[K_NKERNELS] = {"k_make_preseg", "k_cycle_stats(pre+post)", "k_read_qual(pre+post)",
                                                      "k_trim", "k_scan", "k_final", "k_count",
-                                                     "k_cycle_stats(post)", "k_read_qual(post)", "k_kmer_fix",
+                                                     "k_cycle_stats(post residual)", "k_read_qual(post)", "k_kmer_fix",
                                                      "nccl_allreduce(stats)"};
 
 struct fpl_ctx {
@@ -273,10 +275,13 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
         { Timed t(c, K_PRESEG); launch_make_preseg(b, pre, s); }
         { Timed t(c, K_TRIM); launch_trim(c->P, b, st, res, c->d_counters, s);
           if (c->P.opt.adapter_enabled && c->n_adapters > 2) c->launches++; }   // + k_trim_fasta
-        { Timed t(c, K_CYCLE_PRE);
-          if (launch_cycle_stats(&c->cycle_ws, full.seq, full.qual, pre, b.n_reads, tmax, c->d_stats[0], c->C, true,
-                                 ext ? nullptr : c->d_stats[1] + 16 * c->C + FPL_STATS_KMER, c->slots16, s)) return fail("out of device memory (cycle stats workspace)");
-          c->launches += 2; }   // + k_cs_keys and k_cs_gather around the (library) radix sort
+        if (ext) {
+            Timed t(c, K_CYCLE_PRE);
+            if (launch_cycle_stats(&c->cycle_ws, full.seq, full.qual, pre, b.n_reads, tmax, c->d_stats[0], c->C, true, nullptr,
+                                   c->slots16, nullptr, nullptr, nullptr, s))
+                return fail("out of device memory (cycle stats workspace)");
+            c->launches += 2;   // + k_cs_keys and k_cs_gather around the (library) radix sort
+        }
         {
             Timed t(c, K_SCAN);
             if (c->jit.fn) { if (fpl_jit_launch_scan(&c->jit, b, st, s)) return fail("launching k_scan_jit failed"); }
@@ -286,10 +291,18 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
         { Timed t(c, K_FINAL); launch_final(c->P, b, st, res, post, s); }
         if (!ext) {
             { Timed t(c, K_COUNT); launch_count(res, b.n_reads, c->d_counters, true, s); }
-            { Timed t(c, K_CYCLE_POST);
-              if (launch_cycle_stats(&c->cycle_ws, full.seq, full.qual, post, 2 * b.n_reads, tmax, c->d_stats[1], c->C, false, nullptr, false, s))
+            // one pass over the reads counts the pre-filter Stats and, for the read's slot-0 passing segment, the
+            // post-filter per-cycle counters; the residual pass counts the passing segments it did not take
+            { Timed t(c, K_CYCLE_PRE);
+              if (launch_cycle_stats(&c->cycle_ws, full.seq, full.qual, pre, b.n_reads, tmax, c->d_stats[0], c->C, true,
+                                     c->d_stats[1] + 16 * c->C + FPL_STATS_KMER, c->slots16, post, c->d_stats[1], nullptr, s))
                   return fail("out of device memory (cycle stats workspace)");
-          c->launches += 2; }   // + k_cs_keys and k_cs_gather around the (library) radix sort
+              c->launches += 2; }   // + k_cs_keys and k_cs_gather around the (library) radix sort
+            { Timed t(c, K_CYCLE_POST);
+              if (launch_cycle_stats(&c->cycle_ws, full.seq, full.qual, post, 2 * b.n_reads, tmax, c->d_stats[1], c->C, false, nullptr,
+                                     false, nullptr, nullptr, pre, s))
+                  return fail("out of device memory (cycle stats workspace)");
+              c->launches += 2; }   // + k_cs_keys and k_cs_gather around the (library) radix sort
             { Timed t(c, K_KMER_FIX); launch_kmer_fix(b, res, c->d_stats[1] + 16 * c->C + FPL_STATS_KMER, s); }
             { Timed t(c, K_QUAL_PRE); launch_read_qual(b, c->d_stats[0], c->d_stats[1], c->C, res, false, s); }
         } else {
@@ -302,7 +315,8 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
             if (fpl_ext_run(&c->ext, c->P, b, n_bytes, res, c->d_counters, c->d_stats[1], c->C, &fseq, s, xerr, sizeof(xerr)))
                 return fail("--mask/--break stage: %s", xerr);
             { Timed t(c, K_CYCLE_POST);
-              if (launch_cycle_stats(&c->cycle_ws, fseq, full.qual, c->ext.d_stat, c->ext.n_segs, tmax, c->d_stats[1], c->C, true, nullptr, false, s))
+              if (launch_cycle_stats(&c->cycle_ws, fseq, full.qual, c->ext.d_stat, c->ext.n_segs, tmax, c->d_stats[1], c->C, true, nullptr, false,
+                                     nullptr, nullptr, nullptr, s))
                   return fail("out of device memory (cycle stats workspace)");
           c->launches += 2; }   // + k_cs_keys and k_cs_gather around the (library) radix sort
         }

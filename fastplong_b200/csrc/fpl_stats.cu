@@ -8,7 +8,9 @@
 //                 (count << 20 | sum of raw quality chars), laid out so that the 32 lanes of a reduction hit 32 banks
 //                 whatever the segment's misalignment; the tile is flushed once to the global int64 arrays
 //                 mCycleBaseContents / mCycleBaseQual.  The 5-mer variant also fills lane-private 1024-bin tables
-//                 (mKmer) from 2-bit codes packed by multiplication, with an exact A/C/G/T/U test.
+//                 (mKmer) from 2-bit codes packed by multiplication, with an exact A/C/G/T/U test.  Its fused form runs
+//                 over the pre-filter list and counts each read's slot-0 passing segment into the post-filter counters
+//                 too; the plain variant then counts the passing segments it did not take.
 //  k_read_qual    row-shaped: a warp owns a read, builds its quality histogram with shared-memory atomics
 //                 (16-byte vector loads, four per lane in flight), adds it to mBaseQualHistogram and derives the
 //                 per-read median quality (mMedianReadQualHistogram / mMedianReadQualBases / mReads / mLengthSum)
@@ -21,7 +23,7 @@
 #include <stdlib.h>
 #include <cub/cub.cuh>
 
-#define CS_NT_KMER 1024                          // threads per CTA with the 5-mer tables (one CTA per SM: 226 KB of shared memory, within H100's 227 KB per block)
+#define CS_NT_KMER 1024                          // threads per CTA with the 5-mer tables (one CTA per SM: the fused pass takes 214 KB of shared memory, within H100's 227 KB per block)
 #define CS_NT_PLAIN 512
 #define CS_TILE 512                              // bytes of every segment a CTA looks at: one 16-byte vector per lane
 #define CS_ROWW 33                               // words per counter row: 32 lanes + the carry column
@@ -34,7 +36,22 @@
 #define CS_SMEM_BASE (8 * CS_BINW * 4 + CS_STAGE * 16)            // counters + staged descriptors
 #define CS_MBAR_BYTES(NT, DEPTH) (((NT) / 32) * ((DEPTH) + 1) * 8)          // one mbarrier per ring slot (TMA staging)
 #define CS_SMEM_PLAIN (CS_SMEM_BASE + (CS_NT_PLAIN / 32) * (CS_DEPTH_PLAIN + 1) * CS_SLOT + CS_MBAR_BYTES(CS_NT_PLAIN, CS_DEPTH_PLAIN))
-#define CS_SMEM_KMER (CS_SMEM_BASE + (CS_NT_KMER / 32) * (CS_DEPTH_KMER + 1) * CS_SLOT + 1024 * 32 * 4 + CS_MBAR_BYTES(CS_NT_KMER, CS_DEPTH_KMER))   // + lane-private 5-mer tables
+#define CS_KMER_WORDS (512 * 32)                 // lane-private 5-mer tables: [code >> 1][lane], two 16-bit counters per word
+#define CS_SMEM_KMER (CS_SMEM_BASE + (CS_NT_KMER / 32) * (CS_DEPTH_KMER + 1) * CS_SLOT + CS_KMER_WORDS * 4 + CS_MBAR_BYTES(CS_NT_KMER, CS_DEPTH_KMER))
+// The fused pass (pre-filter list, each read carrying its slot-0 post-filter segment [s, e)): the post-filter counters
+// of the columns a tile can reach.  Column pc is the post-filter cycle t0 - 15 - CS_REACH + pc, pc in [0, 16 * CS_PROWW):
+// the pre-filter cycles [t0 - 15, t0 + 512) of the tile, moved back by s < CS_REACH.  The bin stride is a multiple of 32
+// words (the bank of a reduction is its lane's whatever the bin) and CS_PBINW * 4 / 16 fits a dp4a weight byte.
+#define CS_PROWW 62                              // positions per post row
+#define CS_PBINW (16 * CS_PROWW)                 // words per post base bin
+#define CS_REACH (16 * CS_PROWW - CS_TILE - 16)  // 464: post segments starting at s < CS_REACH are counted by the fused pass
+#define CS_SMEM_FUSED (CS_SMEM_KMER + 8 * CS_PBINW * 4 + CS_STAGE * 16)   // + post counters + staged post descriptors
+
+static_assert(CS_PBINW % 32 == 0 && CS_PBINW * 4 / 16 <= 255 && CS_PBINW * 4 % 16 == 0, "post bin stride: banks and dp4a weight");
+static_assert(16 * CS_PROWW >= CS_TILE + 15 + CS_REACH && CS_REACH > 0 && CS_REACH % 16 == 0, "post window covers the reach");
+static_assert(CS_GROUP * 16 <= 0xFFFF, "16-bit 5-mer counter: a lane adds at most 16 5-mers per segment of its group");
+static_assert(CS_GROUP <= 4095 && 127 * CS_GROUP < (1 << 20), "packed counter: a segment adds at most one byte to a column");
+static_assert(CS_SMEM_FUSED <= 232448, "fused pass: one CTA per SM");
 
 namespace {
 
@@ -114,19 +131,23 @@ __device__ __forceinline__ void red_shared_add_imm(uint32_t saddr, uint32_t v) {
 // is column 16*lane + J + S = row (J+S)&15, position lane + ((J+S)>>4).
 //   wm: base & 7 in every byte; qm: quality chars; cw: 0x10 in every byte that counts (0 elsewhere, with qm = 0 there)
 // Per base: one PRMT for the bin, one for the value (quality | 1 << 20), one IMAD for the address, one reduction.
-template <int S, int J>
+// ROWW / BINW: the table's geometry (CS_ROWW / CS_BINW, or CS_PROWW / CS_PBINW for the post window, where S also holds
+// the post shift and runs up to 30).
+template <int S, int J, int ROWW, int BINW>
 __device__ __forceinline__ void count1(const uint32_t (&wm)[4], const uint32_t (&qm)[4], const uint32_t (&cw)[4], uint32_t pk_lane) {
     constexpr int jj = J & 3, m = J + S, z = 8 | jj;                      // selector z: sign fill of a 7-bit byte = 0
     const uint32_t bin = prmt(wm[J >> 2], 0u, jj | z << 4 | z << 8 | z << 12);
     const uint32_t val = prmt(qm[J >> 2], cw[J >> 2], jj | z << 4 | (4 + jj) << 8 | z << 12);
-    red_shared_add_imm<4 * ((m & 15) * CS_ROWW + (m >> 4))>(mad_u32(bin, CS_BINW * 4u, pk_lane), val);
+    red_shared_add_imm<4 * ((m & 15) * ROWW + (m >> 4))>(mad_u32(bin, BINW * 4u, pk_lane), val);
 }
-template <int S>
+template <int S, int ROWW = CS_ROWW, int BINW = CS_BINW>
 __device__ __forceinline__ void count16(const uint32_t (&wm)[4], const uint32_t (&qm)[4], const uint32_t (&cw)[4], uint32_t pk) {
-    count1<S, 0>(wm, qm, cw, pk); count1<S, 1>(wm, qm, cw, pk); count1<S, 2>(wm, qm, cw, pk); count1<S, 3>(wm, qm, cw, pk);
-    count1<S, 4>(wm, qm, cw, pk); count1<S, 5>(wm, qm, cw, pk); count1<S, 6>(wm, qm, cw, pk); count1<S, 7>(wm, qm, cw, pk);
-    count1<S, 8>(wm, qm, cw, pk); count1<S, 9>(wm, qm, cw, pk); count1<S, 10>(wm, qm, cw, pk); count1<S, 11>(wm, qm, cw, pk);
-    count1<S, 12>(wm, qm, cw, pk); count1<S, 13>(wm, qm, cw, pk); count1<S, 14>(wm, qm, cw, pk); count1<S, 15>(wm, qm, cw, pk);
+    count1<S, 0, ROWW, BINW>(wm, qm, cw, pk); count1<S, 1, ROWW, BINW>(wm, qm, cw, pk); count1<S, 2, ROWW, BINW>(wm, qm, cw, pk);
+    count1<S, 3, ROWW, BINW>(wm, qm, cw, pk); count1<S, 4, ROWW, BINW>(wm, qm, cw, pk); count1<S, 5, ROWW, BINW>(wm, qm, cw, pk);
+    count1<S, 6, ROWW, BINW>(wm, qm, cw, pk); count1<S, 7, ROWW, BINW>(wm, qm, cw, pk); count1<S, 8, ROWW, BINW>(wm, qm, cw, pk);
+    count1<S, 9, ROWW, BINW>(wm, qm, cw, pk); count1<S, 10, ROWW, BINW>(wm, qm, cw, pk); count1<S, 11, ROWW, BINW>(wm, qm, cw, pk);
+    count1<S, 12, ROWW, BINW>(wm, qm, cw, pk); count1<S, 13, ROWW, BINW>(wm, qm, cw, pk); count1<S, 14, ROWW, BINW>(wm, qm, cw, pk);
+    count1<S, 15, ROWW, BINW>(wm, qm, cw, pk);
 }
 
 // The same for a vector whose 16 bytes all count (warp-uniform fast path): both operands of the reduction come from
@@ -153,25 +174,75 @@ __device__ __forceinline__ void count16f(const uint32_t (&wb)[4], const uint32_t
     count1f<S, 12>(wb, qm, pk, wa, wv); count1f<S, 13>(wb, qm, pk, wa, wv); count1f<S, 14>(wb, qm, pk, wa, wv); count1f<S, 15>(wb, qm, pk, wa, wv);
 }
 
+// The fused pass: the same value goes to the pre-filter column (m = J + 15, aligned) and to the post-filter window column
+// J + T (T = 15 + (CS_REACH - s) & 15) at the segment's post lane base ppk = window + 4 * (lane + (CS_REACH - s) >> 4);
+// the post bin offset is one more dp4a (wp[j] = (CS_PBINW * 4 / 16) << 8j).  Per base: three dp4a, two reductions.
+template <int T, int J>
+__device__ __forceinline__ void count1ff(const uint32_t (&wb)[4], const uint32_t (&qm)[4], uint32_t pk_lane, uint32_t ppk,
+                                         const uint32_t (&wa)[4], const uint32_t (&wv)[4], const uint32_t (&wp)[4]) {
+    constexpr int jj = J & 3, m = J + 15, mp = J + T;
+    const uint32_t val = __dp4a(qm[J >> 2], wv[jj], 1u << 20);
+    red_shared_add_imm<4 * ((m & 15) * CS_ROWW + (m >> 4))>(__dp4a(wb[J >> 2], wa[jj], pk_lane), val);
+    red_shared_add_imm<4 * ((mp & 15) * CS_PROWW + (mp >> 4))>(__dp4a(wb[J >> 2], wp[jj], ppk), val);
+}
+template <int T>
+__device__ __forceinline__ void count16ff(const uint32_t (&wb)[4], const uint32_t (&qm)[4], uint32_t pk, uint32_t ppk,
+                                          const uint32_t (&wa)[4], const uint32_t (&wv)[4], const uint32_t (&wp)[4]) {
+    count1ff<T, 0>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 1>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 2>(wb, qm, pk, ppk, wa, wv, wp);
+    count1ff<T, 3>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 4>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 5>(wb, qm, pk, ppk, wa, wv, wp);
+    count1ff<T, 6>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 7>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 8>(wb, qm, pk, ppk, wa, wv, wp);
+    count1ff<T, 9>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 10>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 11>(wb, qm, pk, ppk, wa, wv, wp);
+    count1ff<T, 12>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 13>(wb, qm, pk, ppk, wa, wv, wp); count1ff<T, 14>(wb, qm, pk, ppk, wa, wv, wp);
+    count1ff<T, 15>(wb, qm, pk, ppk, wa, wv, wp);
+}
+
 // 0xFF in byte k of the result iff bit k of the nibble n
 __device__ __forceinline__ uint32_t nibble_to_bytes(uint32_t n) { return ((n * 0x00204081u) & 0x01010101u) * 0xFFu; }
 
-// 5-mer ending at byte T of the lane's vector.  P: 2-bit codes, oldest first, the 5-mer's in bits [22-SHL .. 32-SHL); the
-// table word is [code][lane] (no bank conflicts); an invalid 5-mer adds 0 (no branch around the reduction — a reduction
-// predicated on the validity bit is compiled into BSSY / BRA / BSYNC around it: four instructions instead of two).
-// Left shifts as multiplies: they run on the IMAD pipe.  (Right shifts stay shifts: as mul.hi they would use the slower
-// IMAD.HI; mask + shift-and-add compiles to the same four instructions.)
-template <int SHL, int T>
-__device__ __forceinline__ void kmer1(uint32_t P, uint32_t ok, uint32_t km_lane) {
-    const uint32_t idx = (SHL ? mad_u32(P, 1u << SHL, 0u) : P) >> 22;
-    red_shared_add(mad_u32(idx, 128u, km_lane), (ok >> T) & 1u);
+// Post-filter window, masked: the 16 bytes of the lane that lie in [plo, plim) of the tile (vmask as for the pre-filter
+// columns), shift T = S + (CS_REACH - s) & 15 in [0, 30].
+__device__ __forceinline__ void count_post_masked(const uint32_t (&wm)[4], const uint32_t (&q0)[4], int plo, int plim, int T,
+                                                  int lane, uint32_t ppk) {
+    const int lo = max(0, plo - 16 * lane), hi = min(16, max(0, plim - 16 * lane));
+    const uint32_t pm = hi > lo ? ((0xFFFFu >> (16 - hi)) & (0xFFFFu << lo)) : 0u;
+    uint32_t qm[4], cw[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const uint32_t bm = nibble_to_bytes((pm >> (4 * i)) & 15u);
+        qm[i] = q0[i] & bm; cw[i] = 0x10101010u & bm;
+    }
+#define CS_PM(t) case t: count16<t, CS_PROWW, CS_PBINW>(wm, qm, cw, ppk); break;
+    switch (T) {
+        CS_PM(0) CS_PM(1) CS_PM(2) CS_PM(3) CS_PM(4) CS_PM(5) CS_PM(6) CS_PM(7) CS_PM(8) CS_PM(9) CS_PM(10) CS_PM(11) CS_PM(12)
+        CS_PM(13) CS_PM(14) CS_PM(15) CS_PM(16) CS_PM(17) CS_PM(18) CS_PM(19) CS_PM(20) CS_PM(21) CS_PM(22) CS_PM(23) CS_PM(24)
+        CS_PM(25) CS_PM(26) CS_PM(27) CS_PM(28) CS_PM(29) default: count16<30, CS_PROWW, CS_PBINW>(wm, qm, cw, ppk); break;
+    }
+#undef CS_PM
 }
 
-// the same when the 5-mer is known to count: the value is the immediate 1
-template <int SHL>
-__device__ __forceinline__ void kmer1f(uint32_t P, uint32_t km_lane) {
-    const uint32_t idx = (SHL ? mad_u32(P, 1u << SHL, 0u) : P) >> 22;
-    red_shared_add(mad_u32(idx, 128u, km_lane), 1u);
+// 5-mer ending at byte T of the lane's vector.  P: 2-bit codes, oldest first, the 5-mer's in bits [22-SHL .. 32-SHL); the
+// table word is [code >> 1][lane] (no bank conflicts) and holds two 16-bit counters: the low one counts both codes 2w and
+// 2w + 1, the high one code 2w + 1 (the flush takes the difference).  The low bit of the code is bit 1 of byte T
+// (c' = (b >> 1) & 3 of the newest base); hb holds it in every byte, and one PRMT makes the value 1 | bit << 16.
+// An invalid 5-mer adds 0 (no branch around the reduction — a reduction predicated on the validity bit is compiled into
+// BSSY / BRA / BSYNC around it: four instructions instead of two).
+// Left shifts as multiplies: they run on the IMAD pipe.  (Right shifts stay shifts: as mul.hi they would use the slower
+// IMAD.HI; mask + shift-and-add compiles to the same four instructions.)
+template <int T>
+__device__ __forceinline__ uint32_t kmer_inc(const uint32_t (&hb)[4]) {
+    return prmt(hb[T >> 2], 1u, 4 | 5 << 4 | (T & 3) << 8 | 5 << 12);      // byte 0 = 1, byte 2 = the code's low bit
+}
+template <int SHL, int T>
+__device__ __forceinline__ void kmer1(uint32_t P, uint32_t ok, uint32_t km_lane, const uint32_t (&hb)[4]) {
+    const uint32_t w = (SHL ? mad_u32(P, 1u << SHL, 0u) : P) >> 23;
+    red_shared_add(mad_u32(w, 128u, km_lane), mad_u32((ok >> T) & 1u, kmer_inc<T>(hb), 0u));
+}
+
+// the same when the 5-mer is known to count
+template <int SHL, int T>
+__device__ __forceinline__ void kmer1f(uint32_t P, uint32_t km_lane, const uint32_t (&hb)[4]) {
+    const uint32_t w = (SHL ? mad_u32(P, 1u << SHL, 0u) : P) >> 23;
+    red_shared_add(mad_u32(w, 128u, km_lane), kmer_inc<T>(hb));
 }
 
 // Per 4 bytes of sequence: in7 = (nibble of "byte is not one of A, C, G, T, U") << 7, exact for any byte value, and
@@ -188,10 +259,12 @@ __device__ __forceinline__ void encode4(uint32_t w, uint32_t one, uint32_t& nz, 
 
 }  // namespace
 
-// Sorted segment descriptor (by length, longest first): 16 bytes.
+// Sorted segment descriptor (by length, longest first).  The fused pass: the read's slot-0 post-filter segment
+// [ps, ps + pl) relative to the read (pl = 0: none, or one the residual pass counts).
 struct SegD {
     int64_t off;
     int32_t len;
+    int32_t ps, pl;
     int32_t pad;
 };
 // The same as a CTA stages it for its tile: a = 16-byte aligned byte offset of the tile's first vector, lim = how many
@@ -201,6 +274,17 @@ struct __align__(16) TileSeg {
     int32_t lim;
     int32_t sh;
 };
+// The post-filter part (fused pass): the tile bytes [plo, plim) are post-filter cycles; d = CS_REACH - s.  plim <= plo:
+// none in this tile.
+struct __align__(16) TilePost {
+    int32_t plo, plim, d, pad;
+};
+
+// "The fused pass counts this post-filter segment": a passing slot-0 segment starting fewer than CS_REACH bytes into its
+// read.  read_off: the offset of the read's pre-filter segment (the whole read).  The residual pass counts the others.
+__device__ __forceinline__ bool cs_fused_takes(const StatSeg& p, int64_t read_off) {
+    return p.len > 0 && p.slot == 0 && p.off - read_off < CS_REACH;
+}
 
 // DO_KMER: also count the 5-mers; their table is flushed to `stats` and, if given, to `kmer_also` (the post-filter
 // block: post 5-mers = pre 5-mers - the ones k_kmer_fix finds outside the passing segments).
@@ -211,17 +295,22 @@ struct __align__(16) TileSeg {
 // post-filter segment) moves the COLUMNS its bytes count into instead of the bytes (count16<S>).
 // TMA = true: the tile rows are staged by 1-D bulk copies (cp.async.bulk + mbarrier) issued by one lane per warp instead
 // of 32 lanes' cp.async — the variant FPL_CS_TMA=1 selects; both are measured in profiles/README.md.
-template <bool DO_KMER, int NT, int DEPTH, bool TMA>
+// FUSE (5-mer variant over the pre-filter list): every byte of a read's post-filter segment is also counted into the
+// post-filter window at cycle p - s, flushed to `stats_post` — one read of the payload feeds both Stats blocks.
+template <bool DO_KMER, int NT, int DEPTH, bool TMA, bool FUSE>
 __global__ void __launch_bounds__(NT, DO_KMER ? 1 : 2048 / NT / 2)
 k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qualbuf, const SegD* __restrict__ segs,
               int64_t nseg, unsigned long long* __restrict__ stats, int64_t C, unsigned long long* __restrict__ kmer_also,
-              uint32_t one, int aligned) {
+              unsigned long long* __restrict__ stats_post, uint32_t one, int aligned) {
+    static_assert(!FUSE || DO_KMER, "the fused pass is the 5-mer variant");
     extern __shared__ __align__(16) uint8_t cs_smem[];
     uint32_t* packed = reinterpret_cast<uint32_t*>(cs_smem);                       // [8][16][33]: count << 20 | sum of q
     TileSeg* stage = reinterpret_cast<TileSeg*>(cs_smem + 8 * CS_BINW * 4);
     uint8_t* ring = reinterpret_cast<uint8_t*>(stage + CS_STAGE);                  // [warps][DEPTH+1] slots of CS_SLOT bytes
-    uint32_t* kmer = reinterpret_cast<uint32_t*>(ring + (NT / 32) * (DEPTH + 1) * CS_SLOT);   // [1024][32]: one column per lane
-    uint8_t* mbars = reinterpret_cast<uint8_t*>(kmer) + (DO_KMER ? 1024 * 32 * 4 : 0);       // [warps][DEPTH+1] mbarriers (TMA)
+    uint32_t* kmer = reinterpret_cast<uint32_t*>(ring + (NT / 32) * (DEPTH + 1) * CS_SLOT);   // [512][32]: one column per lane
+    uint8_t* mbars = reinterpret_cast<uint8_t*>(kmer) + (DO_KMER ? CS_KMER_WORDS * 4 : 0);    // [warps][DEPTH+1] mbarriers (TMA)
+    uint32_t* ptab = reinterpret_cast<uint32_t*>(mbars + CS_MBAR_BYTES(NT, DEPTH));          // FUSE: [8][16][CS_PROWW]
+    TilePost* pstage = reinterpret_cast<TilePost*>(ptab + (FUSE ? 8 * CS_PBINW : 0));        // FUSE: [CS_STAGE]
     const int wid = threadIdx.x >> 5, lane = lane_id();
     const int64_t t0 = (int64_t)blockIdx.x * CS_TILE;      // first byte of this tile, relative to the aligned segment start
     const int64_t g0 = (int64_t)blockIdx.y * CS_GROUP;
@@ -233,10 +322,13 @@ k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qu
     for (int i = threadIdx.x; i < 8 * CS_BINW; i += NT) packed[i] = 0;
     if (DO_KMER) {
         uint4* kz = reinterpret_cast<uint4*>(kmer);
-        for (int i = threadIdx.x; i < 1024 * 32 / 4; i += NT) kz[i] = make_uint4(0, 0, 0, 0);
+        for (int i = threadIdx.x; i < CS_KMER_WORDS / 4; i += NT) kz[i] = make_uint4(0, 0, 0, 0);
     }
+    if (FUSE)
+        for (int i = threadIdx.x; i < 8 * CS_PBINW; i += NT) ptab[i] = 0;
     const uint32_t pk_lane = shared_addr(packed) + (uint32_t)lane * 4u;
     const uint32_t km_lane = shared_addr(kmer) + (uint32_t)lane * 4u;
+    const uint32_t pt_lane = shared_addr(ptab) + (uint32_t)lane * 4u;
     const uint8_t* seq_lane = seqbuf + 16 * lane;
     const uint8_t* qual_lane = qualbuf + 16 * lane;
     // a slot: [16 bytes in front of the tile][512 bytes of sequence][512 bytes of quality]; the word in front of a lane's
@@ -246,7 +338,9 @@ k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qu
     const uint32_t bar_warp = shared_addr(mbars) + (uint32_t)wid * ((DEPTH + 1) * 8);
     const uint32_t wa[4] = {136u * one, (136u << 8) * one, (136u << 16) * one, (136u << 24) * one};   // one == 1
     const uint32_t wv[4] = {one, one << 8, one << 16, one << 24};
-    uint32_t phase = 0;                                   // TMA: the parity each slot's mbarrier completes next (bit per slot)
+    constexpr uint32_t PW = CS_PBINW * 4 / 16;
+    const uint32_t wp[4] = {PW * one, (PW << 8) * one, (PW << 16) * one, (PW << 24) * one};
+    uint32_t phase = 0;                                  // TMA: the parity each slot's mbarrier completes next (bit per slot)
     if (TMA) {
         if (lane == 0)
             for (int d = 0; d <= DEPTH; d++) mbar_init(bar_warp + 8u * d, 1u);
@@ -267,6 +361,16 @@ k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qu
                 const int64_t lim = (int64_t)ts.sh + sg.len - t0;
                 ts.lim = lim > 0 ? (int32_t)lim : 0;
                 stage[i] = ts;
+                if (FUSE) {
+                    // tile byte of pre-filter cycle c: c + sh - t0
+                    TilePost tp;
+                    const int64_t lo = (int64_t)ts.sh + sg.ps - t0, hi = lo + sg.pl;
+                    tp.plo = lo <= 0 ? 0 : lo >= CS_TILE ? CS_TILE : (int32_t)lo;
+                    tp.plim = sg.pl <= 0 || hi <= 0 ? 0 : hi >= CS_TILE ? CS_TILE : (int32_t)hi;
+                    tp.d = CS_REACH - sg.ps;
+                    tp.pad = 0;
+                    pstage[i] = tp;
+                }
                 reach = sg.len > 0 && (int64_t)sg.len + 15 > t0;
             }
             n += __syncthreads_count(reach);
@@ -323,6 +427,8 @@ k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qu
             const uint32_t sw[4] = {ns.x, ns.y, ns.z, ns.w};
             uint32_t qm[4] = {nq.x, nq.y, nq.z, nq.w};
             const int sh = stage[k].sh, lim = stage[k].lim;
+            TilePost tp = {0, 0, 0, 0};
+            if (FUSE) tp = pstage[k];
             if (kk < n) issue(kk, fill);
             if (!TMA) cp_async_commit();
             kk += NT / 32;
@@ -331,13 +437,29 @@ k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qu
             fill = (fill + 1) & DEPTH;
             if (lim <= 0) continue;                        // warp-uniform: the segment ends in front of this tile
             const bool full = lim >= CS_TILE && t0 != 0;   // warp-uniform: every byte of every lane is a cycle >= 4
+            // FUSE, warp-uniform: the tile holds bytes of the post-filter segment (post), all of its bytes are (pfull);
+            // ppk: the segment's post lane base, T - S: its post shift
+            const bool post = FUSE && tp.plim > tp.plo;
+            const bool pfull = post && tp.plo == 0 && tp.plim >= CS_TILE;
+            const uint32_t ppk = pt_lane + 4u * (uint32_t)(tp.d >> 4);
+            const uint32_t q0[4] = {nq.x, nq.y, nq.z, nq.w};
+            bool post_done = false;
             uint32_t kmask = 0xFFFFu;
             if (full) {
                 // ---- per-(bin, cycle) counters, all 16 bytes of every lane: address and value by dp4a ----
                 const uint32_t wb[4] = {mad_u32(sw[0], 16u, 0u) & 0x70707070u, mad_u32(sw[1], 16u, 0u) & 0x70707070u,
                                         mad_u32(sw[2], 16u, 0u) & 0x70707070u, mad_u32(sw[3], 16u, 0u) & 0x70707070u};
                 // aligned: every segment starts on a 16-byte boundary (the pre-filter pass: whole reads in their slots)
-                if (aligned) count16f<15>(wb, qm, pk_lane, wa, wv);
+                if (FUSE && pfull && (aligned || sh == 0)) {
+                    // both Stats blocks from one value per base
+                    post_done = true;
+#define CS_FF(r) case r: count16ff<15 + r>(wb, qm, pk_lane, ppk, wa, wv, wp); break;
+                    switch (tp.d & 15) {
+                        CS_FF(0) CS_FF(1) CS_FF(2) CS_FF(3) CS_FF(4) CS_FF(5) CS_FF(6) CS_FF(7) CS_FF(8) CS_FF(9) CS_FF(10) CS_FF(11)
+                        CS_FF(12) CS_FF(13) CS_FF(14) default: count16ff<30>(wb, qm, pk_lane, ppk, wa, wv, wp); break;
+                    }
+#undef CS_FF
+                } else if (aligned) count16f<15>(wb, qm, pk_lane, wa, wv);
                 else switch (sh) {
                     case 0: count16f<15>(wb, qm, pk_lane, wa, wv); break;
                     case 1: count16f<14>(wb, qm, pk_lane, wa, wv); break;
@@ -392,6 +514,11 @@ k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qu
                     default: count16<0>(wm, qm, cw, pk_lane); break;
                 }
             }
+            if (FUSE && post && !post_done) {
+                // the tile holds s or e (or the segment is not 16-byte aligned): the post bytes by their own mask
+                const uint32_t wm[4] = {sw[0] & 0x07070707u, sw[1] & 0x07070707u, sw[2] & 0x07070707u, sw[3] & 0x07070707u};
+                count_post_masked(wm, q0, tp.plo, tp.plim, 15 - sh + (tp.d & 15), lane, ppk);
+            }
             if (!DO_KMER) continue;
             // ---- 5-mers ending in this lane's 16 bytes (SURVEY A.1): all five bases in ACGTU, end cycle in [4, len) ----
             // per word: the "not ACGTU" flags and four 2-bit codes c' = (b >> 1) & 3 (A=0, C=1, T/U=2, G=3; the flush maps
@@ -409,29 +536,26 @@ k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qu
             // 20 codes, oldest first, 2 bits each: Phi = codes of bytes -4..11 (32 bits), Plo = bytes 4..15, then 8 zero bits
             const uint32_t Phi = mad_u32(ppc, 1u << 24, mad_u32(pc[0], 1u << 16, mad_u32(pc[1], 256u, pc[2])));
             const uint32_t Plo = mad_u32(pc[1], 1u << 24, mad_u32(pc[2], 1u << 16, pc[3] * 256u));
+            // bit 1 of every byte (the low bit of its code) in bit 0 of the byte: which half of a table word a 5-mer adds to
+            const uint32_t hb[4] = {(sw[0] >> 1) & 0x01010101u, (sw[1] >> 1) & 0x01010101u, (sw[2] >> 1) & 0x01010101u,
+                                    (sw[3] >> 1) & 0x01010101u};
             if (full && !__any_sync(0xffffffffu, (I27 & 0x07FFFF80u) != 0u)) {
-                // plain bases everywhere in the warp's 512 bytes: every 5-mer is counted with the immediate 1
-                kmer1f<0>(Phi, km_lane); kmer1f<2>(Phi, km_lane); kmer1f<4>(Phi, km_lane); kmer1f<6>(Phi, km_lane);
-                kmer1f<8>(Phi, km_lane); kmer1f<10>(Phi, km_lane); kmer1f<12>(Phi, km_lane); kmer1f<14>(Phi, km_lane);
-                kmer1f<16>(Phi, km_lane); kmer1f<18>(Phi, km_lane); kmer1f<20>(Phi, km_lane); kmer1f<22>(Phi, km_lane);
-                kmer1f<8>(Plo, km_lane); kmer1f<10>(Plo, km_lane); kmer1f<12>(Plo, km_lane); kmer1f<14>(Plo, km_lane);
-            } else if (full) {
-                // some lane holds an N (or another byte outside ACGTU): the reductions add the validity bit (a predicated
-                // reduction is compiled into a branch around it: four instructions per 5-mer instead of two)
-                const uint32_t I20 = I27 >> 7;
-                const uint32_t ok = ~(I20 | (I20 >> 1) | (I20 >> 2) | (I20 >> 3) | (I20 >> 4));   // bit t: bytes t-4..t all valid
-                kmer1<0, 0>(Phi, ok, km_lane); kmer1<2, 1>(Phi, ok, km_lane); kmer1<4, 2>(Phi, ok, km_lane); kmer1<6, 3>(Phi, ok, km_lane);
-                kmer1<8, 4>(Phi, ok, km_lane); kmer1<10, 5>(Phi, ok, km_lane); kmer1<12, 6>(Phi, ok, km_lane); kmer1<14, 7>(Phi, ok, km_lane);
-                kmer1<16, 8>(Phi, ok, km_lane); kmer1<18, 9>(Phi, ok, km_lane); kmer1<20, 10>(Phi, ok, km_lane); kmer1<22, 11>(Phi, ok, km_lane);
-                kmer1<8, 12>(Plo, ok, km_lane); kmer1<10, 13>(Plo, ok, km_lane); kmer1<12, 14>(Plo, ok, km_lane); kmer1<14, 15>(Plo, ok, km_lane);
+                // plain bases everywhere in the warp's 512 bytes: every 5-mer counts
+                kmer1f<0, 0>(Phi, km_lane, hb); kmer1f<2, 1>(Phi, km_lane, hb); kmer1f<4, 2>(Phi, km_lane, hb); kmer1f<6, 3>(Phi, km_lane, hb);
+                kmer1f<8, 4>(Phi, km_lane, hb); kmer1f<10, 5>(Phi, km_lane, hb); kmer1f<12, 6>(Phi, km_lane, hb); kmer1f<14, 7>(Phi, km_lane, hb);
+                kmer1f<16, 8>(Phi, km_lane, hb); kmer1f<18, 9>(Phi, km_lane, hb); kmer1f<20, 10>(Phi, km_lane, hb); kmer1f<22, 11>(Phi, km_lane, hb);
+                kmer1f<8, 12>(Plo, km_lane, hb); kmer1f<10, 13>(Plo, km_lane, hb); kmer1f<12, 14>(Plo, km_lane, hb); kmer1f<14, 15>(Plo, km_lane, hb);
             } else {
+                // some lane holds an N (or another byte outside ACGTU), or the segment starts or ends in this tile: the
+                // reductions add the value times the validity bit (a predicated reduction is compiled into a branch around
+                // it: four instructions per 5-mer instead of two)
                 const uint32_t I20 = I27 >> 7;
                 const uint32_t bad = I20 | (I20 >> 1) | (I20 >> 2) | (I20 >> 3) | (I20 >> 4);   // bit t: a byte of t-4..t is invalid
-                const uint32_t ok = ~bad & kmask;
-                kmer1<0, 0>(Phi, ok, km_lane); kmer1<2, 1>(Phi, ok, km_lane); kmer1<4, 2>(Phi, ok, km_lane); kmer1<6, 3>(Phi, ok, km_lane);
-                kmer1<8, 4>(Phi, ok, km_lane); kmer1<10, 5>(Phi, ok, km_lane); kmer1<12, 6>(Phi, ok, km_lane); kmer1<14, 7>(Phi, ok, km_lane);
-                kmer1<16, 8>(Phi, ok, km_lane); kmer1<18, 9>(Phi, ok, km_lane); kmer1<20, 10>(Phi, ok, km_lane); kmer1<22, 11>(Phi, ok, km_lane);
-                kmer1<8, 12>(Plo, ok, km_lane); kmer1<10, 13>(Plo, ok, km_lane); kmer1<12, 14>(Plo, ok, km_lane); kmer1<14, 15>(Plo, ok, km_lane);
+                const uint32_t ok = ~bad & kmask;                                              // kmask = 0xFFFF when full
+                kmer1<0, 0>(Phi, ok, km_lane, hb); kmer1<2, 1>(Phi, ok, km_lane, hb); kmer1<4, 2>(Phi, ok, km_lane, hb); kmer1<6, 3>(Phi, ok, km_lane, hb);
+                kmer1<8, 4>(Phi, ok, km_lane, hb); kmer1<10, 5>(Phi, ok, km_lane, hb); kmer1<12, 6>(Phi, ok, km_lane, hb); kmer1<14, 7>(Phi, ok, km_lane, hb);
+                kmer1<16, 8>(Phi, ok, km_lane, hb); kmer1<18, 9>(Phi, ok, km_lane, hb); kmer1<20, 10>(Phi, ok, km_lane, hb); kmer1<22, 11>(Phi, ok, km_lane, hb);
+                kmer1<8, 12>(Plo, ok, km_lane, hb); kmer1<10, 13>(Plo, ok, km_lane, hb); kmer1<12, 14>(Plo, ok, km_lane, hb); kmer1<14, 15>(Plo, ok, km_lane, hb);
             }
         }
         if (n < CS_STAGE) break;     // the rest of the group is shorter still
@@ -453,9 +577,14 @@ k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qu
     if (DO_KMER) {
         unsigned long long* tail = stats + 16 * C;
         for (int i = threadIdx.x; i < 1024; i += NT) {
+            // word [i >> 1][lane]: low half = codes 2w and 2w + 1, high half = code 2w + 1
             uint32_t sum = 0;
+            const int hi = i & 1;
 #pragma unroll 8
-            for (int l = 0; l < 32; l++) sum += kmer[i * 32 + ((l + threadIdx.x) & 31)];
+            for (int l = 0; l < 32; l++) {
+                const uint32_t v = kmer[(i >> 1) * 32 + ((l + threadIdx.x) & 31)];
+                sum += hi ? v >> 16 : (v & 0xFFFFu) - (v >> 16);
+            }
             if (sum) {
                 // table index: five c' pairs (b2, b1); base2val's code is (b1, b2): swap the bits of every pair
                 const int code = ((i & 0x155) << 1) | ((i >> 1) & 0x155);
@@ -464,21 +593,45 @@ k_cycle_stats(const uint8_t* __restrict__ seqbuf, const uint8_t* __restrict__ qu
             }
         }
     }
+    if (FUSE) {
+        // post window: column 16 * pos + row is the post-filter cycle t0 - 15 - CS_REACH + column
+        unsigned long long* pcontent = stats_post;
+        unsigned long long* pqualsum = stats_post + 8 * C;
+        for (int i = threadIdx.x; i < 8 * CS_PBINW; i += NT) {
+            const uint32_t v = ptab[i];
+            if (v) {
+                const int bin = i / CS_PBINW, p = i % CS_PBINW;
+                const int64_t c = t0 - 15 - CS_REACH + 16 * (p % CS_PROWW) + p / CS_PROWW;
+                const long long cnt = v >> 20, sq = v & 0xFFFFFu;
+                atomicAdd(&pcontent[(int64_t)bin * C + c], (unsigned long long)cnt);
+                atomicAdd(&pqualsum[(int64_t)bin * C + c], (unsigned long long)(sq - 33 * cnt));
+            }
+        }
+    }
 }
 
 namespace {
-__global__ void k_cs_keys(const StatSeg* __restrict__ segs, int64_t n, uint32_t* __restrict__ keys, int32_t* __restrict__ vals) {
+// taken_by (residual pass, or nullptr): the pre-filter list of the fused pass; a segment it counted gets the key 0
+__global__ void k_cs_keys(const StatSeg* __restrict__ segs, int64_t n, uint32_t* __restrict__ keys, int32_t* __restrict__ vals,
+                          const StatSeg* __restrict__ taken_by) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    keys[i] = (uint32_t)max(segs[i].len, 0);
+    const StatSeg s = segs[i];
+    keys[i] = s.len <= 0 || (taken_by && cs_fused_takes(s, taken_by[s.read].off)) ? 0u : (uint32_t)s.len;
     vals[i] = (int32_t)i;
 }
+// post (fused pass, or nullptr): the post-filter list; a read's slot-0 segment [2 * read] rides on its descriptor
 __global__ void k_cs_gather(const StatSeg* __restrict__ segs, const uint32_t* __restrict__ keys, const int32_t* __restrict__ vals,
-                            int64_t n, SegD* __restrict__ out) {
+                            int64_t n, SegD* __restrict__ out, const StatSeg* __restrict__ post) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const StatSeg sg = segs[vals[i]];
     SegD d;
-    d.off = segs[vals[i]].off; d.len = (int32_t)keys[i]; d.pad = 0;
+    d.off = sg.off; d.len = (int32_t)keys[i]; d.ps = 0; d.pl = 0; d.pad = 0;
+    if (post && d.len > 0) {
+        const StatSeg p = post[2 * (int64_t)sg.read];
+        if (cs_fused_takes(p, sg.off)) { d.ps = (int32_t)(p.off - sg.off); d.pl = p.len; }
+    }
     out[i] = d;
 }
 }  // namespace
@@ -489,9 +642,13 @@ void fpl_cycle_ws_free(CycleWs* ws) {
 }
 
 // kmer_also: where the 5-mer counts of this launch go besides `stats` (nullptr = nowhere else); do_kmer = false skips
-// them.  Returns 0, or -1 when the workspace cannot be allocated.
+// them.  fused_post (with do_kmer, segs = the pre-filter list, one per read): the post-filter list; the segments
+// cs_fused_takes accepts are counted into stats_post by the same pass.  residual_of (segs = that post-filter list): the
+// pre-filter list of the fused pass, whose segments this pass skips.  Returns 0, or -1 when the workspace cannot be
+// allocated.
 int launch_cycle_stats(CycleWs* ws, const uint8_t* seq, const uint8_t* qual, const StatSeg* segs, int64_t nseg, int64_t max_len,
                        unsigned long long* stats, int64_t C, bool do_kmer, unsigned long long* kmer_also, bool aligned,
+                       const StatSeg* fused_post, unsigned long long* stats_post, const StatSeg* residual_of,
                        cudaStream_t stream) {
     if (nseg == 0 || max_len <= 0) return 0;
     // the opt-in to more than 48 KB of dynamic shared memory is a per-device function attribute
@@ -500,10 +657,12 @@ int launch_cycle_stats(CycleWs* ws, const uint8_t* seq, const uint8_t* qual, con
     cudaGetDevice(&dev);
     const unsigned long long bit = 1ull << (dev & 63);
     if (!(attr_set.load() & bit)) {
-        if (cudaFuncSetAttribute(k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_KMER) != cudaSuccess ||
-            cudaFuncSetAttribute(k_cycle_stats<false, CS_NT_PLAIN, CS_DEPTH_PLAIN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_PLAIN) != cudaSuccess ||
-            cudaFuncSetAttribute(k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_KMER) != cudaSuccess ||
-            cudaFuncSetAttribute(k_cycle_stats<false, CS_NT_PLAIN, CS_DEPTH_PLAIN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_PLAIN) != cudaSuccess)
+        if (cudaFuncSetAttribute(k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_KMER) != cudaSuccess ||
+            cudaFuncSetAttribute(k_cycle_stats<false, CS_NT_PLAIN, CS_DEPTH_PLAIN, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_PLAIN) != cudaSuccess ||
+            cudaFuncSetAttribute(k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_KMER) != cudaSuccess ||
+            cudaFuncSetAttribute(k_cycle_stats<false, CS_NT_PLAIN, CS_DEPTH_PLAIN, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_PLAIN) != cudaSuccess ||
+            cudaFuncSetAttribute(k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_FUSED) != cudaSuccess ||
+            cudaFuncSetAttribute(k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CS_SMEM_FUSED) != cudaSuccess)
             return -1;
         attr_set.fetch_or(bit);
     }
@@ -533,19 +692,23 @@ int launch_cycle_stats(CycleWs* ws, const uint8_t* seq, const uint8_t* qual, con
         }
     }
     const unsigned blocks = (unsigned)((nseg + 255) / 256);
-    k_cs_keys<<<blocks, 256, 0, stream>>>(segs, nseg, ws->k_in, ws->v_in);
+    k_cs_keys<<<blocks, 256, 0, stream>>>(segs, nseg, ws->k_in, ws->v_in, residual_of);
     size_t bytes = ws->tmp_bytes;
     cub::DeviceRadixSort::SortPairsDescending(ws->tmp, bytes, ws->k_in, ws->k_out, ws->v_in, ws->v_out, (int)nseg, 0, end_bit, stream);
-    k_cs_gather<<<blocks, 256, 0, stream>>>(segs, ws->k_out, ws->v_out, nseg, static_cast<SegD*>(ws->sorted));
+    const bool fuse = do_kmer && fused_post != nullptr;
+    k_cs_gather<<<blocks, 256, 0, stream>>>(segs, ws->k_out, ws->v_out, nseg, static_cast<SegD*>(ws->sorted), fuse ? fused_post : nullptr);
     dim3 grid((unsigned)((max_len + 15 + CS_TILE - 1) / CS_TILE), (unsigned)((nseg + CS_GROUP - 1) / CS_GROUP));
     const SegD* sorted = static_cast<const SegD*>(ws->sorted);
+    const int al = aligned ? 1 : 0;
     static const bool tma = getenv("FPL_CS_TMA") != nullptr && atoi(getenv("FPL_CS_TMA")) != 0;
     if (tma) {
-        if (do_kmer) k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, true><<<grid, CS_NT_KMER, CS_SMEM_KMER, stream>>>(seq, qual, sorted, nseg, stats, C, kmer_also, 1u, aligned ? 1 : 0);
-        else k_cycle_stats<false, CS_NT_PLAIN, CS_DEPTH_PLAIN, true><<<grid, CS_NT_PLAIN, CS_SMEM_PLAIN, stream>>>(seq, qual, sorted, nseg, stats, C, nullptr, 1u, aligned ? 1 : 0);
+        if (fuse) k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, true, true><<<grid, CS_NT_KMER, CS_SMEM_FUSED, stream>>>(seq, qual, sorted, nseg, stats, C, kmer_also, stats_post, 1u, al);
+        else if (do_kmer) k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, true, false><<<grid, CS_NT_KMER, CS_SMEM_KMER, stream>>>(seq, qual, sorted, nseg, stats, C, kmer_also, nullptr, 1u, al);
+        else k_cycle_stats<false, CS_NT_PLAIN, CS_DEPTH_PLAIN, true, false><<<grid, CS_NT_PLAIN, CS_SMEM_PLAIN, stream>>>(seq, qual, sorted, nseg, stats, C, nullptr, nullptr, 1u, al);
     } else {
-        if (do_kmer) k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, false><<<grid, CS_NT_KMER, CS_SMEM_KMER, stream>>>(seq, qual, sorted, nseg, stats, C, kmer_also, 1u, aligned ? 1 : 0);
-        else k_cycle_stats<false, CS_NT_PLAIN, CS_DEPTH_PLAIN, false><<<grid, CS_NT_PLAIN, CS_SMEM_PLAIN, stream>>>(seq, qual, sorted, nseg, stats, C, nullptr, 1u, aligned ? 1 : 0);
+        if (fuse) k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, false, true><<<grid, CS_NT_KMER, CS_SMEM_FUSED, stream>>>(seq, qual, sorted, nseg, stats, C, kmer_also, stats_post, 1u, al);
+        else if (do_kmer) k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, false, false><<<grid, CS_NT_KMER, CS_SMEM_KMER, stream>>>(seq, qual, sorted, nseg, stats, C, kmer_also, nullptr, 1u, al);
+        else k_cycle_stats<false, CS_NT_PLAIN, CS_DEPTH_PLAIN, false, false><<<grid, CS_NT_PLAIN, CS_SMEM_PLAIN, stream>>>(seq, qual, sorted, nseg, stats, C, nullptr, nullptr, 1u, al);
     }
     return 0;
 }
