@@ -307,11 +307,13 @@ k_final(const __grid_constant__ DevParams P, DevBatch b, const ReadState* __rest
     const int wid = threadIdx.x >> 5, lane = lane_id();
     const int64_t r = (int64_t)blockIdx.x * FINAL_WARPS + wid;
     if (r >= b.n_reads) return;
+    // the kernel is a chain of dependent loads per warp: the read's offset is loaded beside its ReadState (not after the
+    // alive test), so that the bytes at the arg-mins are one load away from both
+    const int64_t off = b.offsets[r];
     const ReadState s = st[r];
     fpl_read_result* out = &res[r];
     StatSeg ps0 = {0, 0, -1, 0, 0}, ps1 = ps0;
     if (s.alive) {
-        const int64_t off = b.offsets[r];
         const uint8_t* seq = b.seq + off + s.lo;
         const uint8_t* qual = b.qual + off + s.lo;
         const int L = s.len;
@@ -406,10 +408,10 @@ k_final(const __grid_constant__ DevParams P, DevBatch b, const ReadState* __rest
             }
         }
         if (lane == 0) {
-            uint32_t flags = out->flags;
-            if (split) flags |= FPL_FLAG_MIDDLE_ADAPTER;
-            if (seg0right) flags |= FPL_FLAG_SEG0_IS_RIGHT;
-            out->flags = flags;
+            // k_trim wrote the record's other flags: these are or-ed in without reading it back (a reduction, nothing
+            // for the warp to wait for), and only by the split reads
+            const uint32_t flags = (split ? FPL_FLAG_MIDDLE_ADAPTER : 0u) | (seg0right ? FPL_FLAG_SEG0_IS_RIGHT : 0u);
+            if (flags) atomicOr(&out->flags, flags);
             out->n_segments = nseg;
             for (int k = 0; k < nseg; k++) {
                 out->seg_lo[k] = s.lo + segLo[k];
