@@ -6,7 +6,7 @@ import os
 import numpy as np
 
 from . import abi
-from .abi import FplAdapters, FplBatch, FplOptions, RESULT_DTYPE
+from .abi import FplAdapters, FplBatch, FplOptions, FplOutBatch, RESULT_DTYPE
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libfplgpu.so")
@@ -38,6 +38,7 @@ def load_library():
                                            C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.fpl_emit_fastq_host.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p, C.c_int64,
                                         C.POINTER(C.c_int64)]
+    lib.fpl_emit_batch_device.argtypes = [C.c_void_p, C.POINTER(FplOutBatch), C.POINTER(FplOutBatch)]
     lib.fpl_stream.argtypes = [C.c_void_p]
     lib.fpl_stream.restype = C.c_void_p
     lib.fpl_fetch_results.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
@@ -74,6 +75,7 @@ def load_library():
 
 
 EXPORTS = ["fpl_last_error", "fpl_abi_version", "fpl_create", "fpl_destroy", "fpl_process_host", "fpl_process_device", "fpl_process_fastq_host", "fpl_emit_fastq_host",
+           "fpl_emit_batch_device",
            "fpl_sync", "fpl_stream", "fpl_last_segments", "fpl_last_mask_regions", "fpl_fetch_results", "fpl_stats_cycles", "fpl_stats_reserve", "fpl_stats_download",
            "fpl_stats_device_ptr", "fpl_counter_words", "fpl_counters_download", "fpl_counters_device_ptr",
            "fpl_comm_unique_id", "fpl_comm_init", "fpl_comm_destroy", "fpl_comm_size", "fpl_comm_agree_cycles", "fpl_allreduce_stats",
@@ -87,6 +89,24 @@ class _DeviceArray:
         self.__cuda_array_interface__ = {"shape": (int(n_words),), "typestr": "<i8", "data": (int(ptr), False),
                                          "version": 2}
         self._owner = owner
+
+
+class EmittedBatch:
+    """A packed batch fpl_emit_batch_device wrote into torch tensors: seq / qual (uint8, FPL_BATCH_BYTES(n_bytes) long, or
+    empty when there are no reads), offsets (int64), lens (int32), segs (uint8, 20 bytes per read: abi.SEGMENT_DTYPE)."""
+
+    def __init__(self, seq, qual, offsets, lens, segs, n_bytes):
+        self.seq, self.qual, self.offsets, self.lens, self.segs, self.n_bytes = seq, qual, offsets, lens, segs, int(n_bytes)
+
+    @property
+    def n_reads(self):
+        return int(self.lens.shape[0])
+
+    def to_host(self):
+        """(PackedBatch in host memory, abi.SEGMENT_DTYPE array)"""
+        from .pack import PackedBatch
+        arr = [t.cpu().numpy() for t in (self.seq, self.qual, self.offsets, self.lens, self.segs)]
+        return PackedBatch(*arr[:4]), arr[4].view(abi.SEGMENT_DTYPE)
 
 
 class Engine:
@@ -157,6 +177,36 @@ class Engine:
                                                  C.byref(n_out), failed.ctypes.data if failed.size else None, failed.size,
                                                  C.byref(n_failed)))
         return out.tobytes(), failed.tobytes()
+
+    def emit_batch(self, want_failed=True, device=None):
+        """The output reads of the last process*() call as packed batches in torch tensors on `device` (default: the
+        engine's CUDA device): (out, failed) EmittedBatch objects, failed None unless want_failed (fpl_emit_batch_device).
+        The sizing call, then the copying call, then a sync: the tensors are complete when this returns."""
+        import torch
+        dev = torch.device(device) if device is not None else torch.device("cuda", self.options.device)
+        if dev.type == "cuda" and (dev.index if dev.index is not None else torch.cuda.current_device()) != self.options.device:
+            raise FplError(f"emit_batch: the context runs on cuda:{self.options.device}, not on {dev}")
+        descs = [FplOutBatch() for _ in range(2 if want_failed else 1)]
+        ptrs = [C.byref(d) for d in descs] + [None]
+        rc = self.lib.fpl_emit_batch_device(self.h, ptrs[0], ptrs[1])
+        if rc < 0:
+            self._check(rc)
+        got = []
+        for d in descs:
+            n, nb = int(d.n_reads), int(d.n_bytes)
+            size = abi.batch_bytes(nb) if n else 0
+            b = EmittedBatch(torch.empty(size, dtype=torch.uint8, device=dev), torch.empty(size, dtype=torch.uint8, device=dev),
+                             torch.empty(n, dtype=torch.int64, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
+                             torch.empty(n * abi.SEGMENT_DTYPE.itemsize, dtype=torch.uint8, device=dev), nb)
+            if n:
+                d.seq, d.qual, d.offsets, d.lens, d.segs = (t.data_ptr() for t in (b.seq, b.qual, b.offsets, b.lens, b.segs))
+            d.cap_reads, d.cap_bytes = n, size
+            got.append(b)
+        if dev.type == "cuda":
+            torch.cuda.synchronize(dev)       # the allocations are ordered on torch's stream, the copy on the context's
+        self._check(self.lib.fpl_emit_batch_device(self.h, ptrs[0], ptrs[1]))
+        self.sync()
+        return got[0], (got[1] if want_failed else None)
 
     def process_device(self, seq_ptr, qual_ptr, offsets_ptr, lens_ptr, n_reads, n_bytes, results_ptr=None):
         b = FplBatch(seq_ptr, qual_ptr, offsets_ptr, lens_ptr, n_reads, n_bytes)

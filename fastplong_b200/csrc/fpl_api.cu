@@ -55,13 +55,14 @@ static int fail(const char* fmt, ...) {
         if (e_ != cudaSuccess) return fail("%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
     } while (0)
 
-enum { K_PRESEG, K_CYCLE_PRE, K_QUAL_PRE, K_TRIM, K_SCAN, K_FINAL, K_COUNT, K_CYCLE_POST, K_QUAL_POST, K_KMER_FIX, K_ALLREDUCE, K_NKERNELS };
+enum { K_PRESEG, K_CYCLE_PRE, K_QUAL_PRE, K_TRIM, K_SCAN, K_FINAL, K_COUNT, K_CYCLE_POST, K_QUAL_POST, K_KMER_FIX, K_ALLREDUCE,
+       K_EMIT_BATCH_SIZES, K_EMIT_BATCH_COPY, K_NKERNELS };
 // K_CYCLE_PRE: the fused pass (both Stats blocks) without --mask/--break, the pre-filter pass with it; K_CYCLE_POST: the
 // post-filter segments the fused pass did not take, or the whole --mask/--break post-filter list
 static const char* const kKernelNames[K_NKERNELS] = {"k_make_preseg", "k_cycle_stats(pre+post)", "k_read_qual(pre+post)",
                                                      "k_trim", "k_scan", "k_final", "k_count",
                                                      "k_cycle_stats(post residual)", "k_read_qual(post)", "k_kmer_fix",
-                                                     "nccl_allreduce(stats)"};
+                                                     "nccl_allreduce(stats)", "k_emit_batch(sizes)", "k_emit_batch(copy)"};
 
 struct fpl_ctx {
     int device = 0;
@@ -74,6 +75,9 @@ struct fpl_ctx {
     FplEmit emit;       // device-side output text of the last fpl_process_fastq_host chunk (fpl_emit_fastq_host)
     bool emit_valid = false;            // the last call was a successful fpl_process_fastq_host: chunk + records + results in HBM
     int64_t emit_n = 0;
+    FplBatchEmit bemit;                 // fpl_emit_batch_device: sizes of the output batches of the last fpl_process_* call
+    bool bemit_valid = false;           // the last fpl_process_* call succeeded: bsrc + last_results + ext lists describe it
+    DevBatch bsrc = {};                 // the batch that call processed (the context's staging or the caller's buffers)
     int64_t last_bytes = 0;
     bool slots16 = false;               // this batch's read offsets are multiples of 16 (checked: host and device batches)
     int n_adapters = 0;
@@ -224,6 +228,8 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
     CK(cudaSetDevice(c->device));
     collect_times(c);
     c->emit_valid = false; c->emit.built = false;
+    c->bemit_valid = false; c->bemit.built = false;
+    c->bsrc = full;
     c->last_n = n;
     if (ensure_reads(c, n)) return -1;
     fpl_read_result* d_res = d_res_out ? d_res_out : c->d_results;
@@ -527,6 +533,7 @@ void fpl_destroy(fpl_ctx* c) {
     fpl_ingest_free(&c->ingest);
     fpl_ext_free(&c->ext);
     fpl_emit_free(&c->emit);
+    fpl_emit_batch_free(&c->bemit);
     if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
@@ -534,6 +541,7 @@ void fpl_destroy(fpl_ctx* c) {
 int fpl_process_device(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results_dev) {
     g_err[0] = 0;
     if (!c || !b) return fail("fpl_process_device: null argument");
+    c->bemit_valid = false;
     CK(cudaSetDevice(c->device));
     const int64_t n = b->n_reads;
     if (n < 0) return fail("fpl_process_device: negative n_reads");
@@ -564,9 +572,12 @@ int fpl_process_device(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results_
             CK(cudaMemcpyAsync(c->h_lens.data(), b->lens, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, c->stream));
             CK(cudaStreamSynchronize(c->stream));
         }
-        return run_batch(c, d, c->h_lens.data(), results_dev, b->n_bytes);
+        if (run_batch(c, d, c->h_lens.data(), results_dev, b->n_bytes)) return -1;
+    } else if (run_batch(c, d, nullptr, results_dev, b->n_bytes, nullptr, nullptr, n ? c->h_minmax[1] : 0)) {
+        return -1;
     }
-    return run_batch(c, d, nullptr, results_dev, b->n_bytes, nullptr, nullptr, n ? c->h_minmax[1] : 0);
+    c->bemit_valid = true;
+    return 0;
 }
 
 void* fpl_stream(fpl_ctx* c) { return c ? (void*)c->stream : nullptr; }
@@ -582,6 +593,7 @@ int fpl_sync(fpl_ctx* c) {
 int fpl_process_host(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results) {
     g_err[0] = 0;
     if (!c || !b) return fail("fpl_process_host: null argument");
+    c->bemit_valid = false;
     CK(cudaSetDevice(c->device));
     const int64_t n = b->n_reads;
     if (n < 0 || b->n_bytes < 0) return fail("fpl_process_host: negative size");
@@ -648,6 +660,7 @@ int fpl_process_host(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results) {
     if (n) CK(cudaMemcpyAsync(results, c->d_results, sizeof(fpl_read_result) * n, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
     collect_times(c);
+    c->bemit_valid = true;
     return 0;
 }
 
@@ -655,6 +668,9 @@ int fpl_process_fastq_host(fpl_ctx* c, const uint8_t* text, int64_t n_bytes, int
                            fpl_read_result* results, int64_t max_records, int64_t* n_records, int64_t* consumed) {
     g_err[0] = 0;
     if (!c || !n_records || !consumed || (n_bytes > 0 && !text)) return fail("fpl_process_fastq_host: null argument");
+    // the ingest below overwrites the record table and offsets the batch emit of the last call reads, even when it then
+    // refuses the chunk: nothing is left to emit from until this call succeeds
+    c->bemit_valid = false; c->bemit.built = false;
     if (n_bytes < 0 || n_bytes >= (1ll << 40)) return fail("fpl_process_fastq_host: bad chunk size");
     CK(cudaSetDevice(c->device));
     char err[256] = "";
@@ -664,7 +680,11 @@ int fpl_process_fastq_host(fpl_ctx* c, const uint8_t* text, int64_t n_bytes, int
     if (rc > 0) return 1;
     *n_records = nrec;
     c->emit_valid = false; c->emit.built = false;
-    if (nrec == 0) { c->emit_valid = true; c->emit_n = 0; return 0; }
+    if (nrec == 0) {
+        c->emit_valid = true; c->emit_n = 0;
+        c->bsrc = DevBatch{}; c->bemit_valid = true;
+        return 0;
+    }
     if (nrec > max_records) return 1;
     if (!records || !results) return fail("fpl_process_fastq_host: records/results is null");
     FplIngest& g = c->ingest;
@@ -690,6 +710,7 @@ int fpl_process_fastq_host(fpl_ctx* c, const uint8_t* text, int64_t n_bytes, int
     CK(cudaStreamSynchronize(c->stream));
     collect_times(c);
     c->emit_valid = true; c->emit_n = nrec;
+    c->bemit_valid = true;
     return 0;
 }
 
@@ -704,7 +725,7 @@ int fpl_emit_fastq_host(fpl_ctx* c, int want_failed, uint8_t* out, int64_t out_c
     FplEmit& e = c->emit;
     if (!e.built || e.with_failed != (want_failed != 0)) {
         const bool ext = c->P.opt.mask_enabled || c->P.opt.break_enabled;
-        EmitSource src;
+        EmitSource src = {};
         src.text = c->ingest.d_text; src.rec = c->ingest.d_rec; src.res = c->last_results; src.n_reads = c->emit_n;
         src.segs = ext ? c->ext.d_segs : nullptr;
         src.seg_off = ext ? c->ext.d_off : nullptr;
@@ -721,6 +742,63 @@ int fpl_emit_fastq_host(fpl_ctx* c, int want_failed, uint8_t* out, int64_t out_c
     if (e.out_bytes) CK(cudaMemcpyAsync(out, e.d_out, (size_t)e.out_bytes, cudaMemcpyDeviceToHost, c->stream));
     if (e.failed_bytes) CK(cudaMemcpyAsync(failed, e.d_failed, (size_t)e.failed_bytes, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+// is `o` (an output with n_reads reads in n_bytes bytes) writable?  0 = yes, 1 = too small / missing buffers, -1 = misaligned
+static int out_fits(const fpl_out_batch* o, int64_t n_reads, int64_t n_bytes) {
+    if (n_reads == 0) return 0;
+    if (!o->seq || !o->qual || !o->offsets || !o->lens || o->cap_reads < n_reads || o->cap_bytes < FPL_BATCH_BYTES(n_bytes)) return 1;
+    if ((reinterpret_cast<uintptr_t>(o->seq) | reinterpret_cast<uintptr_t>(o->qual)) & 15) return -1;
+    return 0;
+}
+
+int fpl_emit_batch_device(fpl_ctx* c, fpl_out_batch* out, fpl_out_batch* failed) {
+    g_err[0] = 0;
+    if (!c || !out) return fail("fpl_emit_batch_device: null argument");
+    out->n_reads = out->n_bytes = 0;
+    if (failed) failed->n_reads = failed->n_bytes = 0;
+    if (!c->bemit_valid) return fail("fpl_emit_batch_device: no successful fpl_process_* call to emit from");
+    CK(cudaSetDevice(c->device));
+    const bool ext = c->P.opt.mask_enabled || c->P.opt.break_enabled;
+    EmitSource src = {};
+    src.res = c->last_results; src.n_reads = c->bsrc.n_reads;
+    src.segs = ext ? c->ext.d_segs : nullptr;
+    src.seg_off = ext ? c->ext.d_off : nullptr;
+    src.mseq = (c->P.opt.mask_enabled && c->ext.n_segs > 0) ? c->ext.d_mseq : nullptr;   // fpl_ext_run made the masked copy
+    src.offsets = c->bsrc.offsets; src.seq = c->bsrc.seq; src.qual = c->bsrc.qual;
+    FplBatchEmit& e = c->bemit;
+    if (!e.built) {
+        e.n_out = e.out_bytes = e.n_failed = e.failed_bytes = 0;
+        if (src.n_reads) {
+            char err[256] = "";
+            if (fpl_emit_batch_reserve(&e, src.n_reads, err, sizeof(err))) return fail("fpl_emit_batch_device: %s", err);
+            { Timed t(c, K_EMIT_BATCH_SIZES); launch_emit_batch_sizes(src, e.d_cnt, c->stream); }
+            if (fpl_emit_batch_scan(&e, src.n_reads, c->stream, err, sizeof(err))) return fail("fpl_emit_batch_device: %s", err);
+        }
+        e.built = true;
+    }
+    out->n_reads = e.n_out; out->n_bytes = e.out_bytes;
+    if (failed) { failed->n_reads = e.n_failed; failed->n_bytes = e.failed_bytes; }
+    const int fo = out_fits(out, e.n_out, e.out_bytes), ff = failed ? out_fits(failed, e.n_failed, e.failed_bytes) : 0;
+    if (fo < 0 || ff < 0) return fail("fpl_emit_batch_device: seq and qual must be 16-byte aligned");
+    if (fo || ff) return 1;                 // the sizes stay built: call again with room
+    const bool do_out = e.n_out > 0, do_failed = failed && e.n_failed > 0;
+    if (!do_out && !do_failed) return 0;
+    EmitBatchOut o = {}, f = {};
+    if (do_out) o = EmitBatchOut{out->seq, out->qual, out->offsets, out->lens, out->segs};
+    if (do_failed) f = EmitBatchOut{failed->seq, failed->qual, failed->offsets, failed->lens, failed->segs};
+    // the tail pads; the slots (padding included) are the kernel's
+    if (do_out) {
+        CK(cudaMemsetAsync(out->seq + e.out_bytes, 0, FPL_TAIL_PAD, c->stream));
+        CK(cudaMemsetAsync(out->qual + e.out_bytes, 0, FPL_TAIL_PAD, c->stream));
+    }
+    if (do_failed) {
+        CK(cudaMemsetAsync(failed->seq + e.failed_bytes, 0, FPL_TAIL_PAD, c->stream));
+        CK(cudaMemsetAsync(failed->qual + e.failed_bytes, 0, FPL_TAIL_PAD, c->stream));
+    }
+    { Timed t(c, K_EMIT_BATCH_COPY); launch_emit_batch_copy(src, e.d_off, o, f, c->stream); }
+    CK(cudaGetLastError());
     return 0;
 }
 

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define FPL_ABI_VERSION 5
+#define FPL_ABI_VERSION 6
 
 /* Filter result codes — identical to src/common.h:43-50 (they index FilterResult::mFilterReadStats[32]). */
 enum {
@@ -308,6 +308,42 @@ int fpl_process_fastq_host(fpl_ctx* ctx, const uint8_t* text, int64_t n_bytes, i
  */
 int fpl_emit_fastq_host(fpl_ctx* ctx, int want_failed, uint8_t* out, int64_t out_cap, int64_t* out_bytes,
                         uint8_t* failed, int64_t failed_cap, int64_t* failed_bytes);
+
+/*
+ * SURVEY §8f row 2, device half, for packed batches: the output reads of the LAST fpl_process_* call on this context (host,
+ * device or FASTQ text), cut on the device into packed device batches.  The next fpl_process_* call invalidates them, as it
+ * does fpl_emit_fastq_host's text.  After fpl_process_device the caller's batch buffers and results array must stay valid
+ * and unchanged until the emit has run: the copy reads them.
+ *   out     every passing output read, in the order the --out writer receives them (input order, then segment order within a
+ *           read): split parts, --break pieces, and with --mask the masked bases
+ *   failed  (NULL: none) every read whose only output read failed a filter, as the --failed_out writer receives it: r1 after
+ *           the trims (the record's trim window), its bases masked only if that output read is r1 itself.  A read dropped by
+ *           trimAndCut is in neither batch.
+ * Each is a valid fpl_batch for fpl_process_device: slots contiguous in output order, on 16-byte boundaries,
+ * offsets[j+1] = offsets[j] + round_up(lens[j], 16); n_bytes = the end of the last slot; every byte of
+ * [0, FPL_BATCH_BYTES(n_bytes)) of seq and qual is written (slot padding and tail pad are 0), so equal outputs are equal
+ * buffers.  segs[j] (segs may be NULL) says where output read j came from: read = input read, [lo, lo+len) = the window on
+ * the original read, result = the filter code (the --failed_out reason), median_qual, split_side / break_index = the
+ * name tags of Read::breakByGap / breakByRegions (0 in `failed`: its names carry none), is_r1.
+ * Two phases, like fpl_emit_fastq_host: n_reads / n_bytes of out (and failed) are always set; if an output with reads has a
+ * NULL seq / qual / offsets / lens, cap_reads < n_reads or cap_bytes < FPL_BATCH_BYTES(n_bytes), the call returns 1 and
+ * writes nothing — the sizes stay built on the device, so a second call with room only copies.  That call is
+ * stream-ordered on the context's stream (fpl_sync / fpl_stream order it) and returns without a host synchronisation.
+ * seq and qual must be 16-byte aligned.  An output with n_reads == 0 needs no buffers and is not written.  The copy reads
+ * nothing outside the documented extent of the source batch (see fpl_batch).  Returns 0, 1, or < 0 on error (e.g. no
+ * successful fpl_process_* call since the context was created or since the last failed one).
+ */
+typedef struct fpl_out_batch {        /* all pointers are DEVICE pointers, caller-owned */
+    uint8_t* seq;
+    uint8_t* qual;                    /* cap_bytes each */
+    int64_t* offsets;
+    int32_t* lens;                    /* cap_reads each */
+    fpl_segment* segs;                /* cap_reads, or NULL: where each output read came from */
+    int64_t cap_reads, cap_bytes;     /* in */
+    int64_t n_reads, n_bytes;         /* out: always set */
+} fpl_out_batch;
+
+int fpl_emit_batch_device(fpl_ctx* ctx, fpl_out_batch* out, fpl_out_batch* failed);
 
 /* Output reads / masked regions of the last fpl_process_* call (--mask / --break only; *n = 0 otherwise). */
 int fpl_last_segments(fpl_ctx* ctx, fpl_segment* out, int64_t cap, int64_t* n);
