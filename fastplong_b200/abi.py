@@ -2,7 +2,7 @@
 import ctypes as C
 import numpy as np
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 COMM_ID_BYTES = 128        # FPL_COMM_ID_BYTES == sizeof(ncclUniqueId)
 MAX_ADAPTER_LEN = 1024
 MAX_ADAPTERS = 1024
@@ -70,6 +70,11 @@ class FplOutBatch(C.Structure):
     """fpl_out_batch: a destination of fpl_emit_batch_device (device pointers; n_reads / n_bytes are set by the call)"""
     _fields_ = [("seq", C.c_void_p), ("qual", C.c_void_p), ("offsets", C.c_void_p), ("lens", C.c_void_p), ("segs", C.c_void_p),
                 ("cap_reads", C.c_int64), ("cap_bytes", C.c_int64), ("n_reads", C.c_int64), ("n_bytes", C.c_int64)]
+
+
+class FplReportInfo(C.Structure):
+    """fpl_report_info: what fpl_report_json takes beyond the context's Options"""
+    _fields_ = [("struct_size", C.c_int32), ("is_rna", C.c_int32), ("version", C.c_char_p), ("command", C.c_char_p)]
 
 
 RESULT_DTYPE = np.dtype([

@@ -6,7 +6,7 @@ import os
 import numpy as np
 
 from . import abi
-from .abi import FplAdapters, FplBatch, FplOptions, FplOutBatch, RESULT_DTYPE
+from .abi import FplAdapters, FplBatch, FplOptions, FplOutBatch, FplReportInfo, RESULT_DTYPE
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libfplgpu.so")
@@ -63,6 +63,7 @@ def load_library():
                                            C.POINTER(C.c_int64)]
     lib.fpl_eval_pick_adapter.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_char_p, C.c_int32]
     lib.fpl_reset.argtypes = [C.c_void_p]
+    lib.fpl_report_json.argtypes = [C.c_void_p, C.POINTER(FplReportInfo), C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
     lib.fpl_last_kernel_times.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(C.c_float),
                                           C.POINTER(C.c_int64), C.c_int]
     lib.fpl_launch_count.argtypes = [C.c_void_p]
@@ -79,7 +80,7 @@ EXPORTS = ["fpl_last_error", "fpl_abi_version", "fpl_create", "fpl_destroy", "fp
            "fpl_sync", "fpl_stream", "fpl_last_segments", "fpl_last_mask_regions", "fpl_fetch_results", "fpl_stats_cycles", "fpl_stats_reserve", "fpl_stats_download",
            "fpl_stats_device_ptr", "fpl_counter_words", "fpl_counters_download", "fpl_counters_device_ptr",
            "fpl_comm_unique_id", "fpl_comm_init", "fpl_comm_destroy", "fpl_comm_size", "fpl_comm_agree_cycles", "fpl_allreduce_stats",
-           "fpl_eval_adapter_kmers", "fpl_eval_pick_adapter", "fpl_reset", "fpl_last_kernel_times", "fpl_launch_count", "fpl_set_timing"]
+           "fpl_eval_adapter_kmers", "fpl_eval_pick_adapter", "fpl_report_json", "fpl_reset", "fpl_last_kernel_times", "fpl_launch_count", "fpl_set_timing"]
 
 
 class _DeviceArray:
@@ -277,6 +278,18 @@ class Engine:
     def reset(self):
         self._check(self.lib.fpl_reset(self.h))
 
+    def report_json(self, command="", version="0.4.1", is_rna=False):
+        """fastplong's JSON report (-j) of the accumulators, byte for byte as JsonReporter::report writes it
+        (fpl_report_json): the sizing call builds the text on the device, the second call copies it."""
+        info = FplReportInfo(C.sizeof(FplReportInfo), int(bool(is_rna)), version.encode(), command.encode())
+        n = C.c_int64()
+        rc = self.lib.fpl_report_json(self.h, C.byref(info), None, 0, C.byref(n))
+        if rc < 0:
+            self._check(rc)
+        buf = np.empty(n.value, dtype=np.uint8)
+        self._check(self.lib.fpl_report_json(self.h, C.byref(info), buf.ctypes.data, buf.size, C.byref(n)))
+        return buf.tobytes()
+
     # --- multi-GPU merge (one process per GPU): Stats::merge / FilterResult::merge as NCCL all-reduces ---
     @staticmethod
     def comm_unique_id():
@@ -307,10 +320,11 @@ class Engine:
 
     def kernel_times(self):
         """{kernel name: (total device ms, timed launches)} since set_timing(True)."""
-        names = (C.c_char_p * 16)()
-        ms = (C.c_float * 16)()
-        cnt = (C.c_int64 * 16)()
-        k = self.lib.fpl_last_kernel_times(self.h, names, ms, cnt, 16)
+        cap = 32
+        names = (C.c_char_p * cap)()
+        ms = (C.c_float * cap)()
+        cnt = (C.c_int64 * cap)()
+        k = min(self.lib.fpl_last_kernel_times(self.h, names, ms, cnt, cap), cap)
         return {names[i].decode(): (float(ms[i]), int(cnt[i])) for i in range(k)}
 
     @property

@@ -9,10 +9,12 @@
 #include <string.h>
 #include <time.h>
 #include <algorithm>
+#include <map>
 #include <string>
 #include <vector>
 #include <dlfcn.h>
 #include <nccl.h>
+#include <cub/device/device_scan.cuh>
 #include "fpl_device.cuh"
 #include "fpl_scanplan.h"
 #include "fpl_stats.h"
@@ -38,6 +40,9 @@ int launch_cycle_stats(CycleWs*, const uint8_t*, const uint8_t*, const StatSeg*,
 void launch_kmer_fix(const DevBatch&, const fpl_read_result*, unsigned long long*, cudaStream_t);
 void launch_read_qual(const DevBatch&, unsigned long long*, unsigned long long*, int64_t, fpl_read_result*, bool, cudaStream_t);
 void launch_make_preseg(const DevBatch&, StatSeg*, cudaStream_t);
+void launch_report_cycles(const unsigned long long*, const unsigned long long*, int64_t, unsigned long long*, cudaStream_t);
+void launch_report_sizes(const ReportCurves&, int64_t*, cudaStream_t);
+void launch_report_text(const ReportCurves&, const int64_t*, const uint8_t*, const int64_t*, const int64_t*, int, uint8_t*, cudaStream_t);
 
 static thread_local char g_err[512] = "";
 
@@ -56,13 +61,28 @@ static int fail(const char* fmt, ...) {
     } while (0)
 
 enum { K_PRESEG, K_CYCLE_PRE, K_QUAL_PRE, K_TRIM, K_SCAN, K_FINAL, K_COUNT, K_CYCLE_POST, K_QUAL_POST, K_KMER_FIX, K_ALLREDUCE,
-       K_EMIT_BATCH_SIZES, K_EMIT_BATCH_COPY, K_NKERNELS };
+       K_EMIT_BATCH_SIZES, K_EMIT_BATCH_COPY, K_REPORT_CYCLES, K_REPORT_SIZES, K_REPORT_TEXT, K_NKERNELS };
 // K_CYCLE_PRE: the fused pass (both Stats blocks) without --mask/--break, the pre-filter pass with it; K_CYCLE_POST: the
 // post-filter segments the fused pass did not take, or the whole --mask/--break post-filter list
 static const char* const kKernelNames[K_NKERNELS] = {"k_make_preseg", "k_cycle_stats(pre+post)", "k_read_qual(pre+post)",
                                                      "k_trim", "k_scan", "k_final", "k_count",
                                                      "k_cycle_stats(post residual)", "k_read_qual(post)", "k_kmer_fix",
-                                                     "nccl_allreduce(stats)", "k_emit_batch(sizes)", "k_emit_batch(copy)"};
+                                                     "nccl_allreduce(stats)", "k_emit_batch(sizes)", "k_emit_batch(copy)",
+                                                     "k_report(cycles)", "k_report(sizes)", "k_report(text)"};
+
+// fpl_report_json: the report text of the accumulators as they were when it was built, kept in HBM until a call changes them
+struct FplReport {
+    unsigned long long* d_sum = nullptr;            // k_report_cycles: total_cycles, bases, G+C of each block
+    int64_t* d_size = nullptr; int64_t cap_size = 0;   // bytes of every value
+    int64_t* d_off = nullptr; int64_t cap_off = 0;     // their exclusive sum
+    void* d_tmp = nullptr; int64_t cap_tmp = 0;
+    uint8_t* d_frame = nullptr; int64_t cap_frame = 0;   // piece tables + the host-built frame
+    uint8_t* d_text = nullptr; int64_t cap_text = 0;
+    std::vector<uint8_t> h_frame;
+    bool built = false;
+    std::string key;                                // version, command and is_rna of the built text
+    int64_t n_bytes = 0;
+};
 
 struct fpl_ctx {
     int device = 0;
@@ -81,6 +101,8 @@ struct fpl_ctx {
     int64_t last_bytes = 0;
     bool slots16 = false;               // this batch's read offsets are multiples of 16 (checked: host and device batches)
     int n_adapters = 0;
+    std::vector<std::string> adapter_str;   // fpl_adapters order (the report's adapter names and counted substrings)
+    FplReport rep;
     uint8_t* d_adapters = nullptr;
     int* d_alen = nullptr;
     uint4* d_peq = nullptr;
@@ -150,6 +172,7 @@ static int ensure_reads(fpl_ctx* c, int64_t n) {
 
 static int reserve_cycles(fpl_ctx* c, int64_t need) {
     if (need <= c->C) return 0;
+    c->rep.built = false;
     int64_t nc = c->C ? c->C : 1024;
     while (nc < need) nc *= 2;
     for (int w = 0; w < 2; w++) {
@@ -229,6 +252,7 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
     collect_times(c);
     c->emit_valid = false; c->emit.built = false;
     c->bemit_valid = false; c->bemit.built = false;
+    c->rep.built = false;
     c->bsrc = full;
     c->last_n = n;
     if (ensure_reads(c, n)) return -1;
@@ -393,6 +417,7 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
             return fail("fpl_create: adapter %d is %zu bp, longer than FPL_MAX_ADAPTER_LEN=%d", k, len, FPL_MAX_ADAPTER_LEN);
         }
         h_alen[k] = (int)len;
+        c->adapter_str.push_back(s);
         memcpy(&h_ad[(size_t)k * FPL_MAX_ADAPTER_LEN], s, len);
         const int plen = (int)len < FPL_PATTERN_LEN ? (int)len : FPL_PATTERN_LEN;
         {   // packed 2-bit form for the windowed Hamming search (k_trim), only for ACGT-only adapters of <= 32 bp
@@ -534,6 +559,8 @@ void fpl_destroy(fpl_ctx* c) {
     fpl_ext_free(&c->ext);
     fpl_emit_free(&c->emit);
     fpl_emit_batch_free(&c->bemit);
+    cudaFree(c->rep.d_sum); cudaFree(c->rep.d_size); cudaFree(c->rep.d_off); cudaFree(c->rep.d_tmp); cudaFree(c->rep.d_frame);
+    cudaFree(c->rep.d_text);
     if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
@@ -885,6 +912,7 @@ int fpl_reset(fpl_ctx* c) {
         CK(cudaMemsetAsync(c->d_stats[w], 0, sizeof(unsigned long long) * FPL_STATS_WORDS(c->C), c->stream));
     CK(cudaMemsetAsync(c->d_counters, 0, sizeof(unsigned long long) * c->counter_words, c->stream));
     c->used_cycles = 0;
+    c->rep.built = false;
     return 0;
 }
 
@@ -1019,6 +1047,7 @@ int fpl_allreduce_stats(fpl_ctx* c, int64_t cycles) {
                                              (long long)cycles, (long long)c->used_cycles);
     // rows [b*C, b*C + cycles) of the 16 per-cycle arrays, then the tail; the row pointers depend on this rank's C, the
     // counts do not, so ranks need not share a capacity.  One group = one fused launch.
+    c->rep.built = false;
     Timed t(c, K_ALLREDUCE, false);
     CKN(nccl().GroupStart());
     for (int w = 0; w < 2; w++) {
@@ -1034,3 +1063,265 @@ int fpl_allreduce_stats(fpl_ctx* c, int64_t cycles) {
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------------------
+// fpl_report_json: JsonReporter::report (src/jsonreporter.cpp:11-94) from the device accumulators.  The host builds the
+// frame — every line but the 22 per-cycle curves, from a few hundred scalars — and the kernels of fpl_stats.cu print the
+// curves (O(total_cycles) text) into the same device buffer, between the frame's pieces.
+// ------------------------------------------------------------------------------------------------------------------
+namespace {
+
+struct RepBlock {                      // Stats::summarize's scalars of one block (src/stats.cpp:150-263)
+    long long reads, bases, q20, q30, gc, cycles, lensum;
+    const long long* tail;             // FPL_STATS_TAIL words
+};
+
+std::string gfmt(double v) {           // ostream << double
+    char b[32];
+    snprintf(b, sizeof(b), "%g", v);
+    return b;
+}
+
+std::string dec(long long v) { return std::to_string(v); }
+
+double ratio(long long a, long long b) { return b == 0 ? 0.0 : (double)a / (double)b; }
+
+void summary_part(std::string& s, const char* key, const RepBlock& b) {
+    s += std::string("\t\t\"") + key + "\": {\n";
+    s += "\t\t\t\"total_reads\":" + dec(b.reads) + ",\n";
+    s += "\t\t\t\"total_bases\":" + dec(b.bases) + ",\n";
+    s += "\t\t\t\"q20_bases\":" + dec(b.q20) + ",\n";
+    s += "\t\t\t\"q30_bases\":" + dec(b.q30) + ",\n";
+    s += "\t\t\t\"q20_rate\":" + gfmt(ratio(b.q20, b.bases)) + ",\n";
+    s += "\t\t\t\"q30_rate\":" + gfmt(ratio(b.q30, b.bases)) + ",\n";
+    s += "\t\t\t\"read_mean_length\":" + dec(b.reads == 0 ? 0 : (int)(b.lensum / b.reads)) + ",\n";   // Stats::getMeanLength: int
+    s += "\t\t\t\"gc_content\":" + gfmt(ratio(b.gc, b.bases)) + "\n";
+}
+
+// Stats::reportJson's lines in front of the first curve ("A":[)
+void stats_head(std::string& s, const char* key, const RepBlock& b) {
+    s += std::string("\t\"") + key + "\": {\n";
+    s += "\t\t\"total_reads\": " + dec(b.reads) + ",\n";
+    s += "\t\t\"total_bases\": " + dec(b.bases) + ",\n";
+    s += "\t\t\"q20_bases\": " + dec(b.q20) + ",\n";
+    s += "\t\t\"q30_bases\": " + dec(b.q30) + ",\n";
+    s += "\t\t\"total_cycles\": " + dec(b.cycles) + ",\n";
+    s += "\t\t\"quality_curves\": {\n\t\t\t\"A\":[";
+}
+
+// ... and behind the last one (the content curve "GC"): the 5-mer table (Stats::kmer3 / kmer2 names)
+void stats_tail(std::string& s, const RepBlock& b, bool is_rna) {
+    const char bases[4] = {'A', is_rna ? 'U' : 'T', 'C', 'G'};
+    s += "]\n\t\t},\n\t\t\"kmer_count\": {\n";
+    for (int i = 0; i < 64; i++) {
+        for (int j = 0; j < 16; j++) {
+            const char key[6] = {bases[(i >> 4) & 3], bases[(i >> 2) & 3], bases[i & 3], bases[(j >> 2) & 3], bases[j & 3], 0};
+            s += std::string("\t\t\t\"") + key + "\":" + dec(b.tail[FPL_STATS_KMER + (i << 4) + j]);
+            if (j != 15) s += ",";
+        }
+        s += i != 63 ? ",\n" : "\n";
+    }
+    s += "\t\t}\n\t},\n";
+}
+
+struct ClassComp {                     // classcomp (src/filterresult.h:14-23): by length, then lexicographically
+    bool operator()(const std::string& a, const std::string& b) const {
+        return a.size() != b.size() ? a.size() < b.size() : a < b;
+    }
+};
+
+// The 23 frame pieces around the 22 curves (pre quality A,T,C,G,mean, content A,T,C,G,N,GC, then post): piece j comes
+// in front of curve j, piece 22 behind the last.
+std::vector<std::string> report_frame(const fpl_options& o, const std::vector<std::string>& ad, const long long* cnt,
+                                      const RepBlock b[2], const char* version, const char* command, bool is_rna) {
+    std::vector<std::string> p(23);
+    std::string& s = p[0];
+    s = "{\n\t\"summary\": {\n";
+    s += std::string("\t\t\"fastplong_version\": \"") + version + "\",\n";
+    summary_part(s, "before_filtering", b[0]);
+    s += "\t\t},\n";
+    summary_part(s, "after_filtering", b[1]);
+    s += "\t\t}\n\t},\n";
+    // FilterResult::reportJson (src/filterresult.cpp:120-132)
+    s += "\t\"filtering_result\": {\n";
+    s += "\t\t\"passed_filter_reads\": " + dec(cnt[FPL_CNT_FILTER + FPL_PASS_FILTER]) + ",\n";
+    s += "\t\t\"low_quality_reads\": " + dec(cnt[FPL_CNT_FILTER + FPL_FAIL_QUALITY]) + ",\n";
+    s += "\t\t\"too_many_N_reads\": " + dec(cnt[FPL_CNT_FILTER + FPL_FAIL_N_BASE]) + ",\n";
+    if (o.complexity_enabled) s += "\t\t\"low_complexity_reads\": " + dec(cnt[FPL_CNT_FILTER + FPL_FAIL_COMPLEXITY]) + ",\n";
+    s += "\t\t\"too_short_reads\": " + dec(cnt[FPL_CNT_FILTER + FPL_FAIL_LENGTH]) + ",\n";
+    s += "\t\t\"too_long_reads\": " + dec(cnt[FPL_CNT_FILTER + FPL_FAIL_TOO_LONG]) + "\n";
+    s += "\t},\n";
+    // Options::adapterCuttingEnabled (src/options.cpp:27-33): the FASTA alone does not turn the section on
+    if (o.adapter_enabled && (!ad[0].empty() || !ad[1].empty())) {
+        auto name = [](const std::string& a) { return a.empty() || a == "auto" ? std::string("unspecified") : a; };   // :247-259
+        s += "\t\"adapter_cutting\": {\n";
+        s += "\t\t\"adapter_trimmed_reads\": " + dec(cnt[FPL_CNT_ADAPTER_READS]) + ",\n";
+        s += "\t\t\"adapter_trimmed_bases\": " + dec(cnt[FPL_CNT_ADAPTER_BASES]) + ",\n";
+        s += "\t\t\"read_start_adapter\": \"" + name(ad[0]) + "\",\n";
+        s += "\t\t\"read_end_adapter\": \"" + name(ad[1]) + "\",\n";
+        s += "\t\t\"read_adapter_counts\": {";
+        // FilterResult::mAdapter from the event table, then outputAdaptersJson (src/filterresult.cpp:134-169)
+        std::map<std::string, long long, ClassComp> m;
+        for (size_t k = 0; k < ad.size(); k++)
+            for (int side = 0; side < 2; side++)
+                for (int len = 1; len <= (int)ad[k].size(); len++) {
+                    const long long v = cnt[FPL_CNT_FIXED + ((int64_t)k * 2 + side) * (FPL_MAX_ADAPTER_LEN + 1) + len];
+                    if (v) m[side == 0 ? ad[k].substr(ad[k].size() - len) : ad[k].substr(0, len)] += v;
+                }
+        long long total = 0, reported = 0;
+        for (auto& kv : m) total += kv.second;
+        if (total) {
+            const double dtotal = (double)total;
+            bool first = true;
+            for (auto& kv : m) {
+                if (kv.second / dtotal < 0.01) continue;
+                if (!first) s += ", ";
+                first = false;
+                s += "\"" + kv.first + "\":" + dec(kv.second);
+                reported += kv.second;
+            }
+            if (total - reported > 0) s += std::string(first ? "" : ", ") + "\"others\":" + dec(total - reported);
+        }
+        s += "}\n\t},\n";
+    }
+    // FilterResult::reportPolyXTrimJson (src/filterresult.cpp:187-204): keys are ATCG_BASES, never U
+    if (o.polyx_enabled) {
+        s += "\t\"polyx_trimming\": \t{\n";
+        for (int which = 0; which < 2; which++) {
+            const char* key = which ? "polyx_trimmed_bases" : "polyx_trimmed_reads";
+            const long long* v = cnt + (which ? FPL_CNT_POLYX_BASES : FPL_CNT_POLYX_READS);
+            s += std::string("\t\t\"total_") + key + "\": " + dec(v[0] + v[1] + v[2] + v[3]) + ",\n";
+            s += std::string("\t\t\"") + key + "\":{\"A\": " + dec(v[0]) + ", \"T\": " + dec(v[1]) + ", \"C\": " + dec(v[2]) +
+                 ", \"G\": " + dec(v[3]) + "}";
+            s += which ? "\n\t},\n" : ",\n";
+        }
+    }
+    const std::string t = is_rna ? "U" : "T";
+    const std::string qual_names[5] = {"A", t, "C", "G", "mean"}, content_names[6] = {"A", t, "C", "G", "N", "GC"};
+    for (int w = 0; w < 2; w++) {
+        std::string& head = p[11 * w];
+        stats_head(head, w ? "read_after_filtering" : "read_before_filtering", b[w]);
+        for (int k = 1; k < 11; k++) {
+            std::string& q = p[11 * w + k];
+            if (k < 5) q = "],\n\t\t\t\"" + qual_names[k] + "\":[";
+            else if (k == 5) q = "]\n\t\t},\n\t\t\"content_curves\": {\n\t\t\t\"A\":[";
+            else q = "],\n\t\t\t\"" + content_names[k - 5] + "\":[";
+        }
+        stats_tail(p[11 * w + 11], b[w], is_rna);
+    }
+    p[22] += std::string("\t\"command\": \"") + command + "\"\n}";
+    return p;
+}
+
+int grow_dev(void** ptr, int64_t* cap, int64_t need) {
+    if (need <= *cap) return 0;
+    int64_t n = *cap ? *cap : (1 << 16);
+    while (n < need) n *= 2;
+    cudaFree(*ptr); *ptr = nullptr; *cap = 0;
+    CK(cudaMalloc(ptr, (size_t)n));
+    *cap = n;
+    return 0;
+}
+
+// the text of the accumulators as they are now, into c->rep
+int report_build(fpl_ctx* c, const char* version, const char* command, bool is_rna) {
+    FplReport& r = c->rep;
+    r.built = false;
+    const int64_t C = c->C;
+    cudaStream_t s = c->stream;
+    // 1. total_cycles, bases and G+C of both blocks; the tails and the counters come to the host
+    if (!r.d_sum) CK(cudaMalloc(&r.d_sum, 6 * sizeof(unsigned long long)));
+    unsigned long long sum[6] = {(unsigned long long)C, 0, 0, (unsigned long long)C, 0, 0};
+    CK(cudaMemcpyAsync(r.d_sum, sum, sizeof(sum), cudaMemcpyHostToDevice, s));
+    { Timed t(c, K_REPORT_CYCLES); launch_report_cycles(c->d_stats[0], c->d_stats[1], C, r.d_sum, s); }
+    std::vector<long long> tails(2 * FPL_STATS_TAIL), cnt((size_t)c->counter_words);
+    for (int w = 0; w < 2; w++)
+        CK(cudaMemcpyAsync(tails.data() + w * FPL_STATS_TAIL, c->d_stats[w] + 16 * C, sizeof(long long) * FPL_STATS_TAIL,
+                           cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(cnt.data(), c->d_counters, sizeof(long long) * c->counter_words, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(sum, r.d_sum, sizeof(sum), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    RepBlock b[2];
+    for (int w = 0; w < 2; w++) {
+        const long long* tl = tails.data() + w * FPL_STATS_TAIL;
+        long long q20 = 0, q30 = 0;
+        for (int i = 33 + 20; i < 127; i++) q20 += tl[FPL_STATS_QUALHIST + i];      // Stats::summarize :176-186: c + 33, c < 94
+        for (int i = 33 + 30; i < 127; i++) q30 += tl[FPL_STATS_QUALHIST + i];
+        b[w] = RepBlock{tl[FPL_STATS_READS], (long long)sum[3 * w + 1], q20, q30, (long long)sum[3 * w + 2], (long long)sum[3 * w],
+                        tl[FPL_STATS_LENSUM], tl};
+    }
+    const std::vector<std::string> frame = report_frame(c->P.opt, c->adapter_str, cnt.data(), b, version, command, is_rna);
+    // 2. the size of every value, their exclusive sum (the n + 1st entry: the curves' total)
+    ReportCurves R = {};
+    R.blk[0] = c->d_stats[0]; R.blk[1] = c->d_stats[1]; R.C = C; R.T[0] = b[0].cycles; R.T[1] = b[1].cycles;
+    R.is_rna = is_rna ? 1 : 0;
+    const int64_t n = 11 * (R.T[0] + R.T[1]);
+    if (grow_dev((void**)&r.d_size, &r.cap_size, (int64_t)sizeof(int64_t) * (n + 1))) return -1;
+    if (grow_dev((void**)&r.d_off, &r.cap_off, (int64_t)sizeof(int64_t) * (n + 1))) return -1;
+    CK(cudaMemsetAsync(r.d_size + n, 0, sizeof(int64_t), s));
+    { Timed t(c, K_REPORT_SIZES); launch_report_sizes(R, r.d_size, s); }
+    size_t tb = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, r.d_size, r.d_off, n + 1, s));
+    if (grow_dev(&r.d_tmp, &r.cap_tmp, (int64_t)tb + 256)) return -1;
+    CK(cub::DeviceScan::ExclusiveSum(r.d_tmp, tb, r.d_size, r.d_off, n + 1, s));
+    int64_t end[22];                   // the running sum behind curve j
+    for (int j = 0; j < 22; j++) {
+        const int w = j / 11, k = j % 11;
+        CK(cudaMemcpyAsync(&end[j], r.d_off + (w ? 11 * R.T[0] : 0) + (int64_t)(k + 1) * R.T[w], sizeof(int64_t),
+                           cudaMemcpyDeviceToHost, s));
+    }
+    CK(cudaStreamSynchronize(s));
+    // 3. the frame pieces at their places, the curves between them
+    std::vector<int64_t> src(24), dst(23);
+    int64_t fbytes = 0, shift = 0;
+    for (int j = 0; j < 23; j++) {
+        src[j] = fbytes;
+        dst[j] = (j ? end[j - 1] : 0) + shift;      // behind curve j - 1
+        shift += (int64_t)frame[j].size();
+        fbytes += (int64_t)frame[j].size();
+        if (j < 22) R.shift[j] = shift;
+    }
+    src[23] = fbytes;
+    const int64_t total = end[21] + shift;
+    const size_t tables = sizeof(int64_t) * (24 + 23);
+    r.h_frame.resize(tables + (size_t)fbytes);
+    memcpy(r.h_frame.data(), src.data(), sizeof(int64_t) * 24);
+    memcpy(r.h_frame.data() + sizeof(int64_t) * 24, dst.data(), sizeof(int64_t) * 23);
+    for (int j = 0; j < 23; j++) memcpy(r.h_frame.data() + tables + src[j], frame[j].data(), frame[j].size());
+    if (grow_dev((void**)&r.d_frame, &r.cap_frame, (int64_t)r.h_frame.size())) return -1;
+    if (grow_dev((void**)&r.d_text, &r.cap_text, total)) return -1;
+    CK(cudaMemcpyAsync(r.d_frame, r.h_frame.data(), r.h_frame.size(), cudaMemcpyHostToDevice, s));
+    {
+        Timed t(c, K_REPORT_TEXT);
+        const int64_t* d_src = reinterpret_cast<const int64_t*>(r.d_frame);
+        launch_report_text(R, r.d_off, r.d_frame + tables, d_src, d_src + 24, 23, r.d_text, s);
+        c->launches++;                 // + k_report_frame
+    }
+    CK(cudaGetLastError());
+    r.n_bytes = total;
+    r.built = true;
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int fpl_report_json(fpl_ctx* c, const fpl_report_info* info, uint8_t* out, int64_t cap, int64_t* n_bytes) {
+    g_err[0] = 0;
+    if (!c || !info || !n_bytes) return fail("fpl_report_json: null argument");
+    *n_bytes = 0;
+    if (info->struct_size != (int32_t)sizeof(fpl_report_info))
+        return fail("fpl_report_json: fpl_report_info.struct_size %d != %d (ABI mismatch)", info->struct_size, (int)sizeof(fpl_report_info));
+    if (!info->version || !info->command) return fail("fpl_report_json: version and command must not be null");
+    CK(cudaSetDevice(c->device));
+    std::string key = std::string(info->version) + '\0' + info->command + '\0' + (info->is_rna ? "U" : "T");
+    if (!c->rep.built || c->rep.key != key) {
+        if (report_build(c, info->version, info->command, info->is_rna != 0)) { c->rep.built = false; return -1; }
+        c->rep.key.swap(key);
+    }
+    *n_bytes = c->rep.n_bytes;
+    if (!out || cap < c->rep.n_bytes) return 1;     // the text stays built: call again with room
+    CK(cudaMemcpyAsync(out, c->rep.d_text, (size_t)c->rep.n_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    collect_times(c);
+    return 0;
+}

@@ -1008,3 +1008,185 @@ void launch_make_preseg(const DevBatch& b, StatSeg* segs, cudaStream_t stream) {
     if (b.n_reads == 0) return;
     k_make_preseg<<<(unsigned)((b.n_reads + 255) / 256), 256, 0, stream>>>(b, segs);
 }
+
+// ------------------------------------------------------------------------------------------------------------------
+// The per-cycle curves of the JSON report (fpl_report_json; Stats::summarize src/stats.cpp:150-256 computes them,
+// Stats::reportJson :473-548 prints them with ostream <<, i.e. "%.6g").  A cycle's eleven values depend on that cycle's
+// sixteen counters only, so the text is a per-cycle map and a stream compaction:
+//   k_report_cycles  per Stats block: total_cycles (the first cycle whose count over the 8 bins is 0), total bases, G+C
+//   k_report_sizes   thread per cycle: the bytes of its 11 values (with the ',' behind all but a curve's last)
+//   cub scan         -> where each value starts
+//   k_report_text    thread per cycle: the 11 values at their places; k_report_frame drops the host-built JSON frame
+//                    around the 22 curves
+// ------------------------------------------------------------------------------------------------------------------
+
+// The curve values exactly as the reference's doubles are computed: tot / totq over the 8 bins, IEEE division,
+// round-to-nearest int64 -> double.  curve 0..4: quality A, T (U with is_rna), C, G, mean; 5..10: content A, T (U), C, G,
+// N, GC.  blk is one FPL_STATS_WORDS(C) block.
+__device__ __forceinline__ double report_value(const unsigned long long* blk, int64_t C, int64_t c, int curve, int is_rna) {
+    long long tot = 0, totq = 0;
+    for (int b = 0; b < 8; b++) {
+        tot += (long long)blk[b * C + c];
+        totq += (long long)blk[(8 + b) * C + c];
+    }
+    const double mean = (double)totq / (double)tot;
+    if (curve == 4) return mean;
+    const int tbin = is_rna ? ('U' & 7) : ('T' & 7);
+    if (curve < 4) {
+        const int b = curve == 0 ? ('A' & 7) : curve == 1 ? tbin : curve == 2 ? ('C' & 7) : ('G' & 7);
+        const long long n = (long long)blk[b * C + c];
+        return n == 0 ? mean : (double)(long long)blk[(8 + b) * C + c] / (double)n;
+    }
+    if (curve == 10) return (double)((long long)blk[('G' & 7) * C + c] + (long long)blk[('C' & 7) * C + c]) / (double)tot;
+    const int k = curve - 5;
+    const int b = k == 0 ? ('A' & 7) : k == 1 ? tbin : k == 2 ? ('C' & 7) : k == 3 ? ('G' & 7) : ('N' & 7);
+    return (double)(long long)blk[b * C + c] / (double)tot;
+}
+
+// v as printf("%.6g") / libstdc++'s default ostream << double prints it, into out (at most 12 bytes); returns the length.
+// Integer-only and exact on the domain of the curves: 0 and 2^-64 <= |v| < 10^6.  |v| = m * 2^e2 with a 53-bit m (exact
+// scaling by powers of two), six significant digits = |v| * 10^k = m * 5^k * 2^(e2 + k) in 128 bits, rounded half to even;
+// the decimal exponent estimated from the binary one is corrected by exact comparison with 10^5 and 10^6.
+__device__ __forceinline__ int fmt_g6(double v, char* out) {
+    if (v == 0) { out[0] = '0'; return 1; }
+    int n = 0;
+    double a = v;
+    if (a < 0) { out[n++] = '-'; a = -a; }
+    int e2 = 0;
+    while (a < 2097152.0) { a *= 4294967296.0; e2 -= 32; }              // a in [2^21, 2^53)
+    const int p = 63 - __clzll((long long)(unsigned long long)a);        // its leading bit
+    a *= (double)(1ull << (52 - p));
+    e2 -= 52 - p;
+    const unsigned long long m = (unsigned long long)a;                  // 2^52 <= m < 2^53, |v| = m * 2^e2
+    int E = ((e2 + 52) * 78913) >> 18;                                   // floor(log10(2^(e2+52))), may be 1 short
+    E = E < -21 ? -21 : E > 5 ? 5 : E;
+    unsigned long long q = 0;
+    unsigned __int128 P = 0;
+    int s = 0;
+    for (int it = 0; it < 4; it++) {
+        const int k = 5 - E;                                             // 0 <= k <= 26: 5^k < 2^61
+        unsigned long long p5 = 1;
+        for (int i = 0; i < k; i++) p5 *= 5;
+        P = (unsigned __int128)m * p5;                                   // |v| * 10^k = P * 2^-s
+        s = -(e2 + k);
+        q = s >= 128 ? 0 : (unsigned long long)(P >> s);
+        if (q >= 1000000ull && E < 5) { E++; continue; }
+        if (q < 100000ull && E > -21) { E--; continue; }
+        break;
+    }
+    if (s > 0 && s < 128) {                                              // round half to even
+        const unsigned __int128 rem = P - ((unsigned __int128)q << s), half = (unsigned __int128)1 << (s - 1);
+        if (rem > half || (rem == half && (q & 1))) q++;
+    }
+    if (q >= 1000000ull) { q /= 10; E++; }                               // 999999.5 -> 100000, one decade up
+    char d[6];
+    for (int i = 5; i >= 0; i--) { d[i] = (char)('0' + q % 10); q /= 10; }
+    int nd = 6;
+    while (nd > 1 && d[nd - 1] == '0') nd--;                             // %g drops trailing zeros
+    if (E < -4 || E >= 6) {
+        out[n++] = d[0];
+        if (nd > 1) { out[n++] = '.'; for (int i = 1; i < nd; i++) out[n++] = d[i]; }
+        out[n++] = 'e';
+        out[n++] = E < 0 ? '-' : '+';
+        const int ae = E < 0 ? -E : E;
+        out[n++] = (char)('0' + ae / 10);
+        out[n++] = (char)('0' + ae % 10);
+    } else if (E >= 0) {
+        for (int i = 0; i <= E; i++) out[n++] = d[i];
+        if (nd > E + 1) { out[n++] = '.'; for (int i = E + 1; i < nd; i++) out[n++] = d[i]; }
+    } else {
+        out[n++] = '0'; out[n++] = '.';
+        for (int i = 0; i < -E - 1; i++) out[n++] = '0';
+        for (int i = 0; i < nd; i++) out[n++] = d[i];
+    }
+    return n;
+}
+
+namespace {
+
+// sum[3w + 0] = total_cycles of block w (initialised to C by the host), [3w + 1] = its bases, [3w + 2] = its G + C.  Cycle
+// counts never increase with the cycle, so every count of the block lies before total_cycles.
+__global__ void k_report_cycles(const unsigned long long* __restrict__ pre, const unsigned long long* __restrict__ post, int64_t C,
+                                unsigned long long* __restrict__ sum) {
+    const unsigned long long* blk = blockIdx.y ? post : pre;
+    unsigned long long bases = 0, gc = 0, first = (unsigned long long)C;
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (int64_t)gridDim.x * blockDim.x) {
+        unsigned long long t = 0;
+        for (int b = 0; b < 8; b++) t += blk[b * C + c];
+        bases += t;
+        gc += blk[('G' & 7) * C + c] + blk[('C' & 7) * C + c];
+        if (t == 0 && (unsigned long long)c < first) first = (unsigned long long)c;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        bases += __shfl_down_sync(0xffffffffu, bases, o);
+        gc += __shfl_down_sync(0xffffffffu, gc, o);
+        const unsigned long long f = __shfl_down_sync(0xffffffffu, first, o);
+        first = f < first ? f : first;
+    }
+    if (lane_id() == 0) {
+        unsigned long long* s = sum + 3 * blockIdx.y;
+        if (first < (unsigned long long)C) atomicMin(&s[0], first);
+        if (bases) atomicAdd(&s[1], bases);
+        if (gc) atomicAdd(&s[2], gc);
+    }
+}
+
+// the values of block w live at [base_w + curve * T_w + c) of the size / offset vectors
+__device__ __forceinline__ bool report_cycle(const ReportCurves& R, int64_t i, int& w, int64_t& c) {
+    if (i < R.T[0]) { w = 0; c = i; return true; }
+    if (i < R.T[0] + R.T[1]) { w = 1; c = i - R.T[0]; return true; }
+    return false;
+}
+
+__global__ void k_report_sizes(const ReportCurves R, int64_t* __restrict__ size) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int w; int64_t c;
+    if (!report_cycle(R, i, w, c)) return;
+    const int64_t T = R.T[w], base = w ? 11 * R.T[0] : 0;
+    char buf[16];
+    for (int k = 0; k < 11; k++)
+        size[base + k * T + c] = fmt_g6(report_value(R.blk[w], R.C, c, k, R.is_rna), buf) + (c + 1 < T ? 1 : 0);
+}
+
+// off: exclusive sum of the sizes; curve j (block j / 11, curve j % 11) lands behind frame pieces 0..j: shift[j] bytes of frame
+__global__ void k_report_text(const ReportCurves R, const int64_t* __restrict__ off, uint8_t* __restrict__ text) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int w; int64_t c;
+    if (!report_cycle(R, i, w, c)) return;
+    const int64_t T = R.T[w], base = w ? 11 * R.T[0] : 0;
+    char buf[16];
+    for (int k = 0; k < 11; k++) {
+        const int64_t j = base + k * T + c;
+        uint8_t* dst = text + off[j] + R.shift[11 * w + k];
+        const int n = fmt_g6(report_value(R.blk[w], R.C, c, k, R.is_rna), buf);
+        for (int b = 0; b < n; b++) dst[b] = (uint8_t)buf[b];
+        if (c + 1 < T) dst[n] = ',';
+    }
+}
+
+// frame piece j = frame[src[j], src[j + 1]) goes to text + dst[j]; block j copies piece j
+__global__ void k_report_frame(const uint8_t* __restrict__ frame, const int64_t* __restrict__ src, const int64_t* __restrict__ dst,
+                               uint8_t* __restrict__ text) {
+    const int j = blockIdx.x;
+    for (int64_t b = threadIdx.x; b < src[j + 1] - src[j]; b += blockDim.x) text[dst[j] + b] = frame[src[j] + b];
+}
+
+}  // namespace
+
+void launch_report_cycles(const unsigned long long* pre, const unsigned long long* post, int64_t C, unsigned long long* sum,
+                          cudaStream_t stream) {
+    const int64_t want = (C + 255) / 256;
+    k_report_cycles<<<dim3((unsigned)(want < FPL_NUM_SMS * 8 ? want : FPL_NUM_SMS * 8), 2), 256, 0, stream>>>(pre, post, C, sum);
+}
+
+void launch_report_sizes(const ReportCurves& R, int64_t* size, cudaStream_t stream) {
+    const int64_t n = R.T[0] + R.T[1];
+    if (n) k_report_sizes<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(R, size);
+}
+
+void launch_report_text(const ReportCurves& R, const int64_t* off, const uint8_t* frame, const int64_t* src, const int64_t* dst,
+                        int n_pieces, uint8_t* text, cudaStream_t stream) {
+    k_report_frame<<<n_pieces, 256, 0, stream>>>(frame, src, dst, text);
+    const int64_t n = R.T[0] + R.T[1];
+    if (n) k_report_text<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(R, off, text);
+}

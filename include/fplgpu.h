@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define FPL_ABI_VERSION 6
+#define FPL_ABI_VERSION 7
 
 /* Filter result codes — identical to src/common.h:43-50 (they index FilterResult::mFilterReadStats[32]). */
 enum {
@@ -421,6 +421,36 @@ int fpl_eval_adapter_kmers(int device, const fpl_batch* host_batch, int32_t shif
  */
 int fpl_eval_pick_adapter(const uint32_t* counts, const uint64_t* position_acc, int64_t total, int32_t is_rna, char* adapter,
                           int32_t cap);
+
+/*
+ * SURVEY §8f row 4, second half — JsonReporter::report(FilterResult, preStats, postStats) (src/jsonreporter.cpp:11-94): the
+ * exact bytes of fastplong's JSON report (-j) of this context's accumulators — since fpl_create / fpl_reset, or the job's
+ * totals after fpl_allreduce_stats — under the Options the context was created with plus `info`:
+ *   Stats::summarize (src/stats.cpp:150-256): total_cycles = the first cycle whose count over the 8 base bins is 0;
+ *     total_bases and G+C = the counts before it; q20 / q30 = mBaseQualHistogram[c + 33] for 20 (30) <= c < 94 (index 127 is
+ *     not counted); read_mean_length = lengthSum / reads in integers (0 without reads); the curves as the reference's
+ *     doubles, printed like ostream << double ("%.6g"), by kernels (O(total_cycles) text)
+ *   FilterResult::reportJson / reportAdapterJson / reportPolyXTrimJson (src/filterresult.cpp:120-204): "low_complexity_reads"
+ *     only with -y; "adapter_cutting" only when Options::adapterCuttingEnabled (src/options.cpp:27-33: adapter trimming on and
+ *     the start or end adapter non-empty — an adapter FASTA alone does not count); getReadStartAdapter / getReadEndAdapter
+ *     print "unspecified" for "" and "auto" (:247-259); the adapter count map folds the event table's substrings over the
+ *     adapters in classcomp order, entries below 1 % of the total (a double comparison) go to "others"; "polyx_trimming" only
+ *     with polyX trimming on
+ * Two phases, like fpl_emit_fastq_host: *n_bytes is always set; with out == NULL or cap < *n_bytes the call returns 1 and
+ * writes nothing — the text stays built on the device (for the same info), so a second call with room only copies.  Any later
+ * call that changes the accumulators (fpl_process_*, fpl_reset, fpl_allreduce_stats, fpl_stats_reserve) invalidates the
+ * built text; writes through fpl_stats_device_ptr / fpl_counters_device_ptr are not seen until one of those calls.
+ * Synchronous.  Returns 0, 1, or < 0 on error.  The drop-in binary keeps the reference's own JsonReporter.
+ */
+typedef struct fpl_report_info {
+    int32_t struct_size;              /* = sizeof(fpl_report_info) */
+    int32_t is_rna;                   /* Options::isRNA (Evaluator::evaluateSeqLenAndCheckRNA): the 2nd curve is "U", read from
+                                         bin 'U' & 7, and the 5-mer names use U */
+    const char* version;              /* the "fastplong_version" value (the reference's FASTPLONG_VER) */
+    const char* command;              /* the "command" value, written verbatim */
+} fpl_report_info;
+
+int fpl_report_json(fpl_ctx* ctx, const fpl_report_info* info, uint8_t* out, int64_t cap, int64_t* n_bytes);
 
 /* Zero all accumulators (a fresh ThreadConfig); stream-ordered, asynchronous. */
 int fpl_reset(fpl_ctx* ctx);
