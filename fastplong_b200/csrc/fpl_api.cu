@@ -29,16 +29,22 @@ static_assert(sizeof(fpl_read_result) == 64, "fpl_read_result ABI size");
 static_assert(sizeof(ReadState) == 64, "ReadState size");
 static_assert(sizeof(StatSeg) == 24, "StatSeg size");
 
+#define QH_STRIPES 128      // stripes of k_scan_jit's histogram sums (fpl_scan_jit2_src.h)
+
 // kernel launchers (fpl_trim.cu, fpl_scan.cu, fpl_stats.cu)
 void launch_trim(const DevParams&, const DevBatch&, ReadState*, fpl_read_result*, unsigned long long*, cudaStream_t);
 void launch_scan(const DevParams&, const DevBatch&, ReadState*, cudaStream_t);
 void launch_scan_fast(const DevParams&, const ScanPlan&, const DevBatch&, ReadState*, cudaStream_t);
-void launch_final(const DevParams&, const DevBatch&, const ReadState*, fpl_read_result*, StatSeg*, cudaStream_t);
-void launch_count(const fpl_read_result*, int64_t, unsigned long long*, bool, cudaStream_t);
+void launch_final(const DevParams&, const DevBatch&, const ReadState*, fpl_read_result*, StatSeg*, int32_t*, int*, cudaStream_t);
+void launch_count(const fpl_read_result*, int64_t, unsigned long long*, bool, const int32_t*, unsigned long long*, unsigned long long*,
+                  int64_t, cudaStream_t);
 int launch_cycle_stats(CycleWs*, const uint8_t*, const uint8_t*, const StatSeg*, int64_t, int64_t, unsigned long long*, int64_t,
                         bool, unsigned long long*, bool, const StatSeg*, unsigned long long*, const StatSeg*, cudaStream_t);
 void launch_kmer_fix(const DevBatch&, const fpl_read_result*, unsigned long long*, cudaStream_t);
 void launch_read_qual(const DevBatch&, unsigned long long*, unsigned long long*, int64_t, fpl_read_result*, bool, cudaStream_t);
+void launch_read_qual_exc(const DevBatch&, const ReadState*, const int32_t*, const int*, unsigned long long*, unsigned long long*, int64_t,
+                          fpl_read_result*, cudaStream_t);
+void launch_qhist_fold(const unsigned long long*, int, unsigned long long*, unsigned long long*, int64_t, cudaStream_t);
 void launch_make_preseg(const DevBatch&, StatSeg*, cudaStream_t);
 void launch_report_cycles(const unsigned long long*, const unsigned long long*, int64_t, unsigned long long*, cudaStream_t);
 void launch_report_sizes(const ReportCurves&, int64_t*, cudaStream_t);
@@ -61,14 +67,16 @@ static int fail(const char* fmt, ...) {
     } while (0)
 
 enum { K_PRESEG, K_CYCLE_PRE, K_QUAL_PRE, K_TRIM, K_SCAN, K_FINAL, K_COUNT, K_CYCLE_POST, K_QUAL_POST, K_KMER_FIX, K_ALLREDUCE,
-       K_EMIT_BATCH_SIZES, K_EMIT_BATCH_COPY, K_REPORT_CYCLES, K_REPORT_SIZES, K_REPORT_TEXT, K_NKERNELS };
+       K_EMIT_BATCH_SIZES, K_EMIT_BATCH_COPY, K_REPORT_CYCLES, K_REPORT_SIZES, K_REPORT_TEXT, K_QUAL_EXC, K_QHIST_FOLD, K_NKERNELS };
 // K_CYCLE_PRE: the fused pass (both Stats blocks) without --mask/--break, the pre-filter pass with it; K_CYCLE_POST: the
-// post-filter segments the fused pass did not take, or the whole --mask/--break post-filter list
+// post-filter segments the fused pass did not take, or the whole --mask/--break post-filter list.  K_QUAL_EXC and
+// K_QHIST_FOLD replace K_QUAL_PRE where k_scan_jit counts the quality histograms.
 static const char* const kKernelNames[K_NKERNELS] = {"k_make_preseg", "k_cycle_stats(pre+post)", "k_read_qual(pre+post)",
                                                      "k_trim", "k_scan", "k_final", "k_count",
                                                      "k_cycle_stats(post residual)", "k_read_qual(post)", "k_kmer_fix",
                                                      "nccl_allreduce(stats)", "k_emit_batch(sizes)", "k_emit_batch(copy)",
-                                                     "k_report(cycles)", "k_report(sizes)", "k_report(text)"};
+                                                     "k_report(cycles)", "k_report(sizes)", "k_report(text)",
+                                                     "k_read_qual(exceptions)", "k_qhist_fold"};
 
 // fpl_report_json: the report text of the accumulators as they were when it was built, kept in HBM until a call changes them
 struct FplReport {
@@ -122,6 +130,11 @@ struct fpl_ctx {
     CycleWs cycle_ws;
     StatSeg* d_preseg = nullptr;
     StatSeg* d_postseg = nullptr;
+    // k_scan_jit with the quality histograms (jit.qhist): their striped sums, and k_final's list of the reads whose one
+    // passing segment is not their window (k_read_qual_exc)
+    unsigned long long* d_qstripes = nullptr;
+    int32_t* d_exc = nullptr;
+    int* d_nexc = nullptr;
     int64_t last_n = 0;
     fpl_read_result* last_results = nullptr;  // where the last call's records live (device)
     // staging for host batches
@@ -160,12 +173,13 @@ static int ensure_reads(fpl_ctx* c, int64_t n) {
     if (n <= c->cap_reads) return 0;
     int64_t cap = c->cap_reads ? c->cap_reads : 1024;
     while (cap < n) cap *= 2;
-    cudaFree(c->d_state); cudaFree(c->d_results); cudaFree(c->d_preseg); cudaFree(c->d_postseg);
-    c->d_state = nullptr; c->d_results = nullptr; c->d_preseg = nullptr; c->d_postseg = nullptr; c->cap_reads = 0;
+    cudaFree(c->d_state); cudaFree(c->d_results); cudaFree(c->d_preseg); cudaFree(c->d_postseg); cudaFree(c->d_exc);
+    c->d_state = nullptr; c->d_results = nullptr; c->d_preseg = nullptr; c->d_postseg = nullptr; c->d_exc = nullptr; c->cap_reads = 0;
     CK(cudaMalloc(&c->d_state, sizeof(ReadState) * cap));
     CK(cudaMalloc(&c->d_results, sizeof(fpl_read_result) * cap));
     CK(cudaMalloc(&c->d_preseg, sizeof(StatSeg) * cap));
     CK(cudaMalloc(&c->d_postseg, sizeof(StatSeg) * 2 * cap));
+    if (c->jit.qhist) CK(cudaMalloc(&c->d_exc, sizeof(int32_t) * cap));
     c->cap_reads = cap;
     return 0;
 }
@@ -272,6 +286,10 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
     // tiles of reads whose payload stays L2-resident across the kernels that revisit it
     const bool ext = c->P.opt.mask_enabled || c->P.opt.break_enabled;   // variable number of output reads: one tile
     c->ext.n_segs = 0; c->ext.n_regs = 0;
+    // the scan counts the quality histograms (k_scan_jit built with them; never with --mask/--break): k_final lists the
+    // exceptions, k_read_qual_exc treats them, k_count adds the per-read sums and the striped sums are folded at the end
+    const bool qhist = c->jit.fn && c->jit.qhist;
+    if (qhist && n > 0) CK(cudaMemsetAsync(c->d_qstripes, 0, sizeof(unsigned long long) * QH_STRIPES * 256, c->stream));
     int64_t r0 = 0;
     size_t piece = 0;
     while (r0 < n) {
@@ -318,9 +336,13 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
             else if (c->plan.fast) launch_scan_fast(c->P, c->plan, b, st, s);
             else launch_scan(c->P, b, st, s);
         }
-        { Timed t(c, K_FINAL); launch_final(c->P, b, st, res, post, s); }
+        int32_t* exc = qhist ? c->d_exc + r0 : nullptr;
+        if (qhist) CK(cudaMemsetAsync(c->d_nexc, 0, sizeof(int), s));
+        { Timed t(c, K_FINAL); launch_final(c->P, b, st, res, post, exc, c->d_nexc, s); }
         if (!ext) {
-            { Timed t(c, K_COUNT); launch_count(res, b.n_reads, c->d_counters, true, s); }
+            if (qhist) { Timed t(c, K_QUAL_EXC); launch_read_qual_exc(b, st, exc, c->d_nexc, c->d_stats[0], c->d_stats[1], c->C, res, s); }
+            { Timed t(c, K_COUNT);
+              launch_count(res, b.n_reads, c->d_counters, true, b.lens, qhist ? c->d_stats[0] : nullptr, c->d_stats[1], c->C, s); }
             // one pass over the reads counts the pre-filter Stats and, for the read's slot-0 passing segment, the
             // post-filter per-cycle counters; the residual pass counts the passing segments it did not take
             { Timed t(c, K_CYCLE_PRE);
@@ -334,14 +356,14 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
                   return fail("out of device memory (cycle stats workspace)");
               c->launches += 2; }   // + k_cs_keys and k_cs_gather around the (library) radix sort
             { Timed t(c, K_KMER_FIX); launch_kmer_fix(b, res, c->d_stats[1] + 16 * c->C + FPL_STATS_KMER, s); }
-            { Timed t(c, K_QUAL_PRE); launch_read_qual(b, c->d_stats[0], c->d_stats[1], c->C, res, false, s); }
+            if (!qhist) { Timed t(c, K_QUAL_PRE); launch_read_qual(b, c->d_stats[0], c->d_stats[1], c->C, res, false, s); }
         } else {
             // --mask / --break: k_final left the output reads of the adapter stage in the records; fpl_ext_run breaks /
             // masks / filters them (variable count) and the post-filter Stats run over its segment list
             char xerr[256] = "";
             const uint8_t* fseq = full.seq;
             { Timed t(c, K_QUAL_PRE); launch_read_qual(b, c->d_stats[0], c->d_stats[1], c->C, res, true, s); }
-            { Timed t(c, K_COUNT); launch_count(res, b.n_reads, c->d_counters, false, s); }
+            { Timed t(c, K_COUNT); launch_count(res, b.n_reads, c->d_counters, false, nullptr, nullptr, nullptr, 0, s); }
             if (fpl_ext_run(&c->ext, c->P, b, n_bytes, res, c->d_counters, c->d_stats[1], c->C, &fseq, s, xerr, sizeof(xerr)))
                 return fail("--mask/--break stage: %s", xerr);
             { Timed t(c, K_CYCLE_POST);
@@ -352,6 +374,7 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
         }
         r0 = r1;
     }
+    if (qhist && n > 0) { Timed t(c, K_QHIST_FOLD); launch_qhist_fold(c->d_qstripes, QH_STRIPES, c->d_stats[0], c->d_stats[1], c->C, c->stream); }
     CK(cudaGetLastError());
     return 0;
 }
@@ -516,11 +539,21 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
     if (c->plan.fast && getenv("FPL_NO_JIT") == nullptr) {
         char jerr[512] = "";
         const bool doCounts = opt->qual_filter_enabled || opt->length_filter_enabled;
+        // the quality histograms ride on the scan where it loads the quality bytes anyway (the quality or the length
+        // filter) and without --mask/--break (whose post-filter reads are not the windows).  With -Q -L the scan would
+        // load them for the histograms alone: measured on an H100 (profiles/README.md), that loses on 1 kb reads
+        const bool doQhist = doCounts && !(opt->mask_enabled || opt->break_enabled);
         if (fpl_jit_build_scan(c->device, ad->start ? ad->start : "", ad->end ? ad->end : "", opt->adapter_enabled != 0,
-                               doCounts, opt->complexity_enabled != 0, opt->qualified_qual, &c->jit, jerr, sizeof(jerr))) {
+                               doCounts, opt->complexity_enabled != 0, doQhist, opt->qualified_qual, &c->jit, jerr, sizeof(jerr))) {
             fprintf(stderr, "libfplgpu: run-time specialisation unavailable (%s); using the precompiled k_scan_fast\n", jerr);
             c->jit.fn = nullptr;
+            c->jit.qhist = false;
         }
+    }
+    if (c->jit.qhist) {
+        CKC(cudaMalloc(&c->d_qstripes, sizeof(unsigned long long) * QH_STRIPES * 256));
+        CKC(cudaMalloc(&c->d_nexc, sizeof(int)));
+        c->P.qstripes = c->d_qstripes;
     }
     stamp("scan kernel specialisation");
     const char* tb = getenv("FPL_TILE_MBASES");
@@ -554,6 +587,7 @@ void fpl_destroy(fpl_ctx* c) {
     cudaFree(c->d_agree); if (c->h_agree) cudaFreeHost(c->h_agree);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     cudaFree(c->d_state); cudaFree(c->d_results); cudaFree(c->d_preseg); cudaFree(c->d_postseg);
+    cudaFree(c->d_qstripes); cudaFree(c->d_exc); cudaFree(c->d_nexc);
     cudaFree(c->d_seq); cudaFree(c->d_qual); cudaFree(c->d_offsets); cudaFree(c->d_lens);
     fpl_ingest_free(&c->ingest);
     fpl_ext_free(&c->ext);

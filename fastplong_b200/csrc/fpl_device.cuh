@@ -25,6 +25,7 @@ struct DevParams {
     int small_adapters;       // size class of -s / -e: 0 both <= 32 bp, 1 both <= 64 bp, 2 any (k_trim<CLS>)
     int fasta_class;          // the same for the FASTA adapters (k_trim_fasta<CLS>)
     uint32_t one;             // 1: the multiplier of the IMADs that must stay on the FMA pipe (an add the compiler cannot fold)
+    unsigned long long* qstripes;   // k_scan_jit's histogram sums (k_trim hands the address on in the ReadState), else nullptr
 };
 
 // Device view of a packed batch.
@@ -40,10 +41,11 @@ struct DevBatch {
 struct ReadState {
     int32_t lo, len;          // r1 window after trimAndCut / polyX / adapter trims
     uint32_t alive;           // 0 if dropped by trimAndCut
-    uint32_t pad;
+    uint32_t pad;             // k_scan_jit with the quality histograms: the read's median quality char
     unsigned long long best[2];   // middle-adapter scan: (minHamming << 32) | pos, ~0ull = no position scanned
     int32_t lowq, nn, totalq, diff;  // passFilter counts over the window
-    int32_t reserved[4];
+    int32_t reserved[4];      // k_scan_jit with the quality histograms: [0] the window's median quality char (out);
+                              // [1] the read's length, [2..3] DevParams::qstripes (in, written by k_trim)
 };
 
 // A segment to be fed to the Stats kernels: absolute byte offset into the batch buffers + length (0 = skip).

@@ -113,12 +113,14 @@ extern "C" const char* fpl_jit_debug_source(const char* a0, const char* a1) {
     return keep.c_str();
 }
 
-int fpl_jit_build_scan(int device, const char* a0, const char* a1, bool doAdapters, bool doCounts, bool doCplx, int qq,
-                       FplJitKernel* out, char* err, size_t errlen) {
+int fpl_jit_build_scan(int device, const char* a0, const char* a1, bool doAdapters, bool doCounts, bool doCplx, bool doQhist,
+                       int qq, FplJitKernel* out, char* err, size_t errlen) {
     out->fn = nullptr;
+    out->qhist = false;
     std::string defs;
     if (!doAdapters) { a0 = ""; a1 = ""; }
     const bool v1 = getenv("FPL_JIT_V1") != nullptr;       // the round-1 kernel, kept for A/B measurements
+    if (v1) doQhist = false;                                // (version 1 has no histograms)
     defs += std::string("#define FPL_A0 \"") + a0 + "\"\n";
     defs += std::string("#define FPL_A1 \"") + a1 + "\"\n";
     defs += "#define FPL_ALEN0 " + std::to_string(strlen(a0)) + "\n";
@@ -127,13 +129,14 @@ int fpl_jit_build_scan(int device, const char* a0, const char* a1, bool doAdapte
     defs += std::string("#define FPL_DO_ADAPTERS ") + (doAdapters ? "true" : "false") + "\n";
     defs += std::string("#define FPL_DO_COUNTS ") + (doCounts ? "true" : "false") + "\n";
     defs += std::string("#define FPL_DO_CPLX ") + (doCplx ? "true" : "false") + "\n";
+    defs += std::string("#define FPL_DO_QHIST ") + (doQhist ? "true" : "false") + "\n";
     defs += "#define FPL_QQ " + std::to_string(qq & 0x7f) + "\n";
     const char* mb = getenv("FPL_JIT_MINBLOCKS");   // occupancy knob (registers per thread); 8 (64 registers) on H100: 6/8/10 blocks -> 15.1/15.0/23.2 ms (profiles/README.md)
     defs += std::string("#define FPL_MINBLOCKS ") + (mb && atoi(mb) > 0 ? std::to_string(atoi(mb)) : std::string("8")) + "\n";
     const std::string key = std::to_string(device) + "|" + defs;
     std::lock_guard<std::mutex> lock(g_mu);
     auto it = g_cache.find(key);
-    if (it != g_cache.end()) { out->fn = (void*)it->second.fn; return 0; }
+    if (it != g_cache.end()) { out->fn = (void*)it->second.fn; out->qhist = doQhist; return 0; }
 
     const std::string src = defs + (v1 ? std::string(kScanJitSource) : scan_source_v2(a0, a1));
     nvrtcProgram prog;
@@ -170,6 +173,7 @@ int fpl_jit_build_scan(int device, const char* a0, const char* a1, bool doAdapte
     }
     g_cache[key] = c;
     out->fn = (void*)c.fn;
+    out->qhist = doQhist;
     return 0;
 }
 
@@ -180,7 +184,7 @@ int fpl_jit_launch_scan(const FplJitKernel* k, const DevBatch& b, ReadState* st,
     const int64_t* offsets = b.offsets;
     int64_t n = b.n_reads;
     // `one` is the multiplier of the IMADs that must stay IMADs (an add the compiler cannot see through stays on the
-    // FMA pipe); version 1 ignores the extra argument
+    // FMA pipe); version 1 ignores the extra argument.  The histogram inputs (qhist) ride in the ReadState (k_trim).
     unsigned one = 1;
     void* args[] = {(void*)&seq, (void*)&qual, (void*)&offsets, (void*)&st, (void*)&n, (void*)&one};
     // one CTA per read: the hardware scheduler balances the gamma-distributed read lengths better than persistent CTAs

@@ -299,11 +299,12 @@ __device__ Counts count_range(const fpl_options& o, uint32_t one, const uint8_t*
 
 // CLS: size class of -s / -e (DevParams::small_adapters): 0 = both <= 32 bp — the kernel is then compiled without the
 // 128-bit and multi-word Myers forms and their local arrays, which would otherwise set its register budget and occupancy
-// (it is bound by the latency of its dependent loads)
-template <int CLS>
+// (it is bound by the latency of its dependent loads).  QH: k_scan_jit counted the quality histograms, k_final hands the
+// window's median on and lists the other reads in exc (a separate instance: the other paths run the kernel as it was)
+template <int CLS, bool QH>
 __global__ void __launch_bounds__(FINAL_WARPS * 32)
 k_final(const __grid_constant__ DevParams P, DevBatch b, const ReadState* __restrict__ st,
-        fpl_read_result* __restrict__ res, StatSeg* __restrict__ postseg) {
+        fpl_read_result* __restrict__ res, StatSeg* __restrict__ postseg, int32_t* __restrict__ exc, int* __restrict__ n_exc) {
     const int wid = threadIdx.x >> 5, lane = lane_id();
     const int64_t r = (int64_t)blockIdx.x * FINAL_WARPS + wid;
     if (r >= b.n_reads) return;
@@ -313,6 +314,7 @@ k_final(const __grid_constant__ DevParams P, DevBatch b, const ReadState* __rest
     const ReadState s = st[r];
     fpl_read_result* out = &res[r];
     StatSeg ps0 = {0, 0, -1, 0, 0}, ps1 = ps0;
+    bool one_window = false;                             // the read's one passing segment is its window
     if (s.alive) {
         const uint8_t* seq = b.seq + off + s.lo;
         const uint8_t* qual = b.qual + off + s.lo;
@@ -419,29 +421,52 @@ k_final(const __grid_constant__ DevParams P, DevBatch b, const ReadState* __rest
                 out->seg_result[k] = (uint8_t)code[k];
             }
         }
+        // k_scan_jit counted the quality histograms (QH): the window's median is the median of a read whose
+        // one passing segment is the window
+        one_window = !split && nseg == 1 && code[0] == FPL_PASS_FILTER;
+        if (QH && lane == 0) out->pre_median_qual = (uint8_t)s.pad;          // the scan's median of the whole read
+        if (QH && lane == 0 && one_window) out->seg_median_qual[0] = (uint8_t)s.reserved[0];
         if (nseg > 0 && code[0] == FPL_PASS_FILTER) { ps0.off = off + s.lo + segLo[0]; ps0.len = segLen[0]; ps0.read = (int)r; ps0.slot = 0; }
         if (nseg > 1 && code[1] == FPL_PASS_FILTER) { ps1.off = off + s.lo + segLo[1]; ps1.len = segLen[1]; ps1.read = (int)r; ps1.slot = 1; }
         // a passing zero-length segment cannot exist (passFilter fails rlen == 0), so len == 0 <=> "no segment"
     }
     if (lane == 0) { postseg[2 * r] = ps0; postseg[2 * r + 1] = ps1; }
+    // every other read (not alive, split, or a failing segment) goes to k_read_qual_exc's list: one atomic per read
+    if (QH && lane == 0 && !one_window) exc[atomicAdd(n_exc, 1)] = (int32_t)r;
 }
 
+// exc / n_exc (nullptr: k_scan_jit did not count the quality histograms): the list of the reads k_read_qual_exc treats
 void launch_final(const DevParams& P, const DevBatch& b, const ReadState* st, fpl_read_result* res, StatSeg* postseg,
-                  cudaStream_t stream) {
+                  int32_t* exc, int* n_exc, cudaStream_t stream) {
     if (b.n_reads == 0) return;
     unsigned grid = (unsigned)((b.n_reads + FINAL_WARPS - 1) / FINAL_WARPS);
-    if (P.small_adapters == 0) k_final<0><<<grid, FINAL_WARPS * 32, 0, stream>>>(P, b, st, res, postseg);
-    else k_final<2><<<grid, FINAL_WARPS * 32, 0, stream>>>(P, b, st, res, postseg);
+    if (exc) {
+        if (P.small_adapters == 0) k_final<0, true><<<grid, FINAL_WARPS * 32, 0, stream>>>(P, b, st, res, postseg, exc, n_exc);
+        else k_final<2, true><<<grid, FINAL_WARPS * 32, 0, stream>>>(P, b, st, res, postseg, exc, n_exc);
+    } else {
+        if (P.small_adapters == 0) k_final<0, false><<<grid, FINAL_WARPS * 32, 0, stream>>>(P, b, st, res, postseg, exc, n_exc);
+        else k_final<2, false><<<grid, FINAL_WARPS * 32, 0, stream>>>(P, b, st, res, postseg, exc, n_exc);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // k_count: FilterResult counters (src/filterresult.cpp:22-81) from the finished records; block-level
 // aggregation in shared memory, one global atomic per non-zero counter per block.
+// stats_pre != nullptr (k_scan_jit counted the quality histograms): also the per-read sums of both Stats blocks
+// (mReads, mLengthSum, mMedianReadQualHistogram, mMedianReadQualBases, src/stats.cpp:362-374) — every read for the
+// pre-filter block, every passing segment for the post-filter one — which k_read_qual adds on the other paths.
 // ------------------------------------------------------------------------------------------------------------------
+#define CNT_SUMS (2 + 2 * 128)       // per Stats block: reads, length sum, median histogram, median bases
+
 __global__ void __launch_bounds__(256)
-k_count(const fpl_read_result* __restrict__ res, int64_t n, unsigned long long* __restrict__ counters, bool count_segments) {
+k_count(const fpl_read_result* __restrict__ res, int64_t n, unsigned long long* __restrict__ counters, bool count_segments,
+        const int32_t* __restrict__ lens, unsigned long long* __restrict__ stats_pre, unsigned long long* __restrict__ stats_post,
+        int64_t C) {
     __shared__ unsigned long long sh[FPL_CNT_FIXED];
+    __shared__ unsigned long long sums[2][CNT_SUMS];
     for (int i = threadIdx.x; i < FPL_CNT_FIXED; i += blockDim.x) sh[i] = 0;
+    if (stats_pre)
+        for (int i = threadIdx.x; i < 2 * CNT_SUMS; i += blockDim.x) (&sums[0][0])[i] = 0;
     __syncthreads();
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r < n) {
@@ -457,14 +482,46 @@ k_count(const fpl_read_result* __restrict__ res, int64_t n, unsigned long long* 
         }
         if (flags & FPL_FLAG_DROPPED_BY_CUT) atomicAdd(&sh[FPL_CNT_DROPPED], 1ull);
         if (flags & FPL_FLAG_MIDDLE_ADAPTER) atomicAdd(&sh[FPL_CNT_SPLIT], 1ull);
+        if (stats_pre) {
+            // the same order of effects as Stats::statRead: a read counts, its median only when it has bases
+            const int L = lens[r];
+            atomicAdd(&sums[0][0], 1ull);
+            atomicAdd(&sums[0][1], (unsigned long long)L);
+            if (L > 0) {
+                atomicAdd(&sums[0][2 + o->pre_median_qual], 1ull);
+                atomicAdd(&sums[0][2 + 128 + o->pre_median_qual], (unsigned long long)L);
+            }
+            for (int k = 0; k < nseg; k++) {
+                if (o->seg_result[k] != FPL_PASS_FILTER) continue;
+                const int sl = o->seg_len[k];
+                atomicAdd(&sums[1][0], 1ull);
+                atomicAdd(&sums[1][1], (unsigned long long)sl);
+                if (sl > 0) {
+                    atomicAdd(&sums[1][2 + o->seg_median_qual[k]], 1ull);
+                    atomicAdd(&sums[1][2 + 128 + o->seg_median_qual[k]], (unsigned long long)sl);
+                }
+            }
+        }
     }
     __syncthreads();
     for (int i = threadIdx.x; i < FPL_CNT_FIXED; i += blockDim.x)
         if (sh[i]) atomicAdd(&counters[i], sh[i]);
+    if (stats_pre)
+        for (int i = threadIdx.x; i < 2 * CNT_SUMS; i += blockDim.x) {
+            const int w = i / CNT_SUMS, j = i % CNT_SUMS;
+            const unsigned long long v = sums[w][j];
+            if (!v) continue;
+            unsigned long long* tail = (w ? stats_post : stats_pre) + 16 * C;
+            const int at = j == 0 ? FPL_STATS_READS : j == 1 ? FPL_STATS_LENSUM : j < 2 + 128 ? FPL_STATS_MEDHIST + (j - 2)
+                                                                                                : FPL_STATS_MEDBASES + (j - 2 - 128);
+            atomicAdd(&tail[at], v);
+        }
 }
 
-// count_segments = false: --mask/--break, where the output reads are counted by k_ext_filter instead
-void launch_count(const fpl_read_result* res, int64_t n, unsigned long long* counters, bool count_segments, cudaStream_t stream) {
+// count_segments = false: --mask/--break, where the output reads are counted by k_ext_filter instead.  stats_pre /
+// stats_post / C (stats_pre == nullptr: not here): see k_count.
+void launch_count(const fpl_read_result* res, int64_t n, unsigned long long* counters, bool count_segments, const int32_t* lens,
+                  unsigned long long* stats_pre, unsigned long long* stats_post, int64_t C, cudaStream_t stream) {
     if (n == 0) return;
-    k_count<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(res, n, counters, count_segments);
+    k_count<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(res, n, counters, count_segments, lens, stats_pre, stats_post, C);
 }

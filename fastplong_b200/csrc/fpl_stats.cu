@@ -873,18 +873,30 @@ __device__ __forceinline__ void hist_bytes(uint32_t hbase, const uint8_t* qp, in
 // objects.  COOP = false: one warp owns the read.  COOP = true: the whole block does (an ultra-long read streamed by
 // one warp is bound by the latency of that warp's loads); every thread of the block calls it for the same read, the
 // histograms are warp 0's, warp 0 does the medians.
-template <bool COOP>
+// EXC (k_read_qual_exc, a read k_final listed): k_scan_jit has already counted an alive read's whole histogram into the
+// pre-filter sums and its window's into the post-filter ones, and set its pre-filter median.  Such a read histograms its
+// window instead of the whole read, takes it out of the post-filter sums (block_sub) and counts its passing segments
+// as above, relative to the window; a read that is not alive gets the pre-filter part in full.  The per-read sums
+// (reads, lengths, median histograms) are k_count's in this mode.
+template <bool COOP, bool EXC = false>
 __device__ __forceinline__ void read_qual_one(const DevBatch& b, int64_t r, uint32_t* hfull, uint32_t* hseg, uint32_t (*block_hist)[128],
                                               unsigned long long (*block_misc)[2], unsigned long long* const* tail,
-                                              fpl_read_result* __restrict__ res, bool pre_only) {
+                                              fpl_read_result* __restrict__ res, bool pre_only,
+                                              const ReadState* __restrict__ st = nullptr, uint32_t* block_sub = nullptr) {
     const int lane = lane_id(), wid = threadIdx.x >> 5;
     const int me = COOP ? (int)threadIdx.x : lane, nth = COOP ? (int)blockDim.x : 32;
     auto sync = [] { if (COOP) __syncthreads(); else __syncwarp(); };
     const bool lead = !COOP || wid == 0;                 // the warp that owns the medians and the flushes
     const uint32_t hfull_s = shared_addr(hfull), hseg_s = shared_addr(hseg);
-    const uint8_t* qp = b.qual + b.offsets[r];
-    const int L = b.lens[r];
+    const int Lread = b.lens[r];
     fpl_read_result* o = &res[r];
+    bool win = false;                                    // EXC: hfull is the window [w0, w0 + L) of an alive read
+    int w0 = 0, L = Lread;
+    if (EXC) {
+        const ReadState s = st[r];
+        if (s.alive) { win = true; w0 = s.lo; L = s.len; }
+    }
+    const uint8_t* qp = b.qual + b.offsets[r] + w0;
     sync();
     for (int i = me; i < 128; i += nth) hfull[i] = 0;
     sync();
@@ -892,24 +904,33 @@ __device__ __forceinline__ void read_qual_one(const DevBatch& b, int64_t r, uint
     sync();
     uint32_t own[4];
     if (lead) {
-        const uint8_t med = hist_median(hfull, L, lane, own);
+        if (win) {
+            own[0] = hfull[4 * lane]; own[1] = hfull[4 * lane + 1]; own[2] = hfull[4 * lane + 2]; own[3] = hfull[4 * lane + 3];
 #pragma unroll
-        for (int k = 0; k < 4; k++)
-            if (own[k]) atomicAdd(&block_hist[0][4 * lane + k], own[k]);
-        if (lane == 0) {
-            atomicAdd(&block_misc[0][0], 1ull);
-            atomicAdd(&block_misc[0][1], (unsigned long long)L);
-            if (L > 0) {
-                atomicAdd(&tail[0][FPL_STATS_MEDHIST + med], 1ull);
-                atomicAdd(&tail[0][FPL_STATS_MEDBASES + med], (unsigned long long)L);
+            for (int k = 0; k < 4; k++)
+                if (own[k]) atomicAdd(&block_sub[4 * lane + k], own[k]);
+        } else {
+            const uint8_t med = hist_median(hfull, L, lane, own);
+#pragma unroll
+            for (int k = 0; k < 4; k++)
+                if (own[k]) atomicAdd(&block_hist[0][4 * lane + k], own[k]);
+            if (lane == 0) {
+                if (!EXC) {
+                    atomicAdd(&block_misc[0][0], 1ull);
+                    atomicAdd(&block_misc[0][1], (unsigned long long)L);
+                    if (L > 0) {
+                        atomicAdd(&tail[0][FPL_STATS_MEDHIST + med], 1ull);
+                        atomicAdd(&tail[0][FPL_STATS_MEDBASES + med], (unsigned long long)L);
+                    }
+                }
+                o->pre_median_qual = med;
             }
-            o->pre_median_qual = med;
         }
     }
     const int nseg = pre_only ? 0 : o->n_segments;   // --mask/--break: the post-filter part is k_ext_seg_qual's
     for (int k = 0; k < nseg; k++) {
         if (o->seg_result[k] != FPL_PASS_FILTER) continue;      // uniform
-        const int a = o->seg_lo[k], n = o->seg_len[k];
+        const int a = o->seg_lo[k] - w0, n = o->seg_len[k];
         sync();
         if (L - n <= n) {            // copy the read's histogram and take the removed ends out
             for (int i = me; i < 128; i += nth) hseg[i] = hfull[i];
@@ -928,11 +949,13 @@ __device__ __forceinline__ void read_qual_one(const DevBatch& b, int64_t r, uint
             for (int j = 0; j < 4; j++)
                 if (own[j]) atomicAdd(&block_hist[1][4 * lane + j], own[j]);
             if (lane == 0) {
-                atomicAdd(&block_misc[1][0], 1ull);
-                atomicAdd(&block_misc[1][1], (unsigned long long)n);
-                if (n > 0) {
-                    atomicAdd(&tail[1][FPL_STATS_MEDHIST + smed], 1ull);
-                    atomicAdd(&tail[1][FPL_STATS_MEDBASES + smed], (unsigned long long)n);
+                if (!EXC) {
+                    atomicAdd(&block_misc[1][0], 1ull);
+                    atomicAdd(&block_misc[1][1], (unsigned long long)n);
+                    if (n > 0) {
+                        atomicAdd(&tail[1][FPL_STATS_MEDHIST + smed], 1ull);
+                        atomicAdd(&tail[1][FPL_STATS_MEDBASES + smed], (unsigned long long)n);
+                    }
                 }
                 o->seg_median_qual[k] = smed;
             }
@@ -993,6 +1016,73 @@ void launch_read_qual(const DevBatch& b, unsigned long long* stats_pre, unsigned
     const int64_t want = (b.n_reads + RQ_WARPS - 1) / RQ_WARPS;
     const unsigned grid = (unsigned)(want < FPL_NUM_SMS * 64 ? want : FPL_NUM_SMS * 64);
     k_read_qual<<<grid, RQ_WARPS * 32, 0, stream>>>(b, stats_pre, stats_post, C, res, pre_only);
+}
+
+// k_read_qual's work for the reads k_final listed (exc[0, *n_exc)) when k_scan_jit counted the quality histograms: the
+// exceptions to "the read's one passing segment is its window" (see read_qual_one<_, true>).  The grid is capped and the
+// count is read on the device.  block_sub: the windows' histograms, taken out of the post-filter sums.
+__global__ void __launch_bounds__(RQ_WARPS * 32)
+k_read_qual_exc(DevBatch b, const ReadState* __restrict__ st, const int32_t* __restrict__ exc, const int* __restrict__ n_exc,
+                unsigned long long* __restrict__ stats_pre, unsigned long long* __restrict__ stats_post, int64_t C,
+                fpl_read_result* __restrict__ res) {
+    __shared__ uint32_t hist[RQ_WARPS][2][128];
+    __shared__ uint32_t block_hist[2][128];
+    __shared__ uint32_t block_sub[128];
+    __shared__ int n_long;
+    __shared__ long long long_read[RQ_LIST];
+    const int wid = threadIdx.x >> 5, lane = lane_id();
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) (&block_hist[0][0])[i] = 0;
+    for (int i = threadIdx.x; i < 128; i += blockDim.x) block_sub[i] = 0;
+    if (threadIdx.x == 0) n_long = 0;
+    __syncthreads();
+    unsigned long long* tail[2] = {stats_pre + 16 * C, stats_post + 16 * C};
+    const int64_t n = *n_exc;
+    const int64_t nwarps = (int64_t)gridDim.x * RQ_WARPS;
+    for (int64_t i = (int64_t)blockIdx.x * RQ_WARPS + wid; i < n; i += nwarps) {
+        const int64_t r = exc[i];
+        if (b.lens[r] > RQ_LONG) {
+            int slot = -1;
+            if (lane == 0) slot = atomicAdd(&n_long, 1);
+            slot = __shfl_sync(0xffffffffu, slot, 0);
+            if (slot < RQ_LIST) { if (lane == 0) long_read[slot] = r; continue; }
+        }
+        read_qual_one<false, true>(b, r, hist[wid][0], hist[wid][1], block_hist, nullptr, tail, res, false, st, block_sub);
+    }
+    __syncthreads();
+    const int nl = min(n_long, RQ_LIST);
+    for (int i = 0; i < nl; i++)
+        read_qual_one<true, true>(b, long_read[i], hist[0][0], hist[0][1], block_hist, nullptr, tail, res, false, st, block_sub);
+    __syncthreads();
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) {
+        const int which = i >> 7, bin = i & 127;
+        if (block_hist[which][bin]) atomicAdd(&tail[which][FPL_STATS_QUALHIST + bin], (unsigned long long)block_hist[which][bin]);
+    }
+    for (int i = threadIdx.x; i < 128; i += blockDim.x)
+        if (block_sub[i]) atomicAdd(&tail[1][FPL_STATS_QUALHIST + i], 0ull - (unsigned long long)block_sub[i]);
+}
+
+void launch_read_qual_exc(const DevBatch& b, const ReadState* st, const int32_t* exc, const int* n_exc, unsigned long long* stats_pre,
+                          unsigned long long* stats_post, int64_t C, fpl_read_result* res, cudaStream_t stream) {
+    if (b.n_reads == 0) return;
+    // the list is a few percent of the reads: a grid of a few blocks per SM, capped by what the whole batch would need
+    const int64_t want = (b.n_reads + RQ_WARPS - 1) / RQ_WARPS;
+    const unsigned grid = (unsigned)(want < FPL_NUM_SMS * 8 ? want : FPL_NUM_SMS * 8);
+    k_read_qual_exc<<<grid, RQ_WARPS * 32, 0, stream>>>(b, st, exc, n_exc, stats_pre, stats_post, C, res);
+}
+
+// the striped sums of k_scan_jit's histograms ([QH_STRIPES][2][128]: whole reads, windows) -> mBaseQualHistogram of the
+// pre-filter and of the post-filter block; one thread per (block, bin)
+__global__ void k_qhist_fold(const unsigned long long* __restrict__ stripes, int n_stripes, unsigned long long* __restrict__ stats_pre,
+                             unsigned long long* __restrict__ stats_post, int64_t C) {
+    const int i = threadIdx.x;           // 256 threads
+    unsigned long long sum = 0;
+    for (int k = 0; k < n_stripes; k++) sum += stripes[(int64_t)k * 256 + i];
+    if (sum) atomicAdd(&((i >> 7) ? stats_post : stats_pre)[16 * C + FPL_STATS_QUALHIST + (i & 127)], sum);
+}
+
+void launch_qhist_fold(const unsigned long long* stripes, int n_stripes, unsigned long long* stats_pre, unsigned long long* stats_post,
+                       int64_t C, cudaStream_t stream) {
+    k_qhist_fold<<<1, 256, 0, stream>>>(stripes, n_stripes, stats_pre, stats_post, C);
 }
 
 // pre-stats segment list: every input read, full length

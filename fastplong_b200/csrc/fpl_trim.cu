@@ -661,7 +661,11 @@ k_trim(const __grid_constant__ DevParams P, DevBatch b, ReadState* __restrict__ 
         s.lo = w.lo; s.len = w.len; s.alive = alive ? 1u : 0u; s.pad = 0;
         s.best[0] = ~0ull; s.best[1] = ~0ull;
         s.lowq = s.nn = s.totalq = s.diff = 0;
-        s.reserved[0] = s.reserved[1] = s.reserved[2] = s.reserved[3] = 0;
+        // k_scan_jit with the quality histograms takes the read's length and where to add them from here (its
+        // arguments are the adapters' scan's)
+        s.reserved[0] = 0; s.reserved[1] = L;
+        s.reserved[2] = (int32_t)(uint32_t)reinterpret_cast<uintptr_t>(P.qstripes);
+        s.reserved[3] = (int32_t)(uint32_t)(reinterpret_cast<uintptr_t>(P.qstripes) >> 32);
         st[r] = s;
         if (!alive) out->flags |= FPL_FLAG_DROPPED_BY_CUT;
         else { out->trim_lo = w.lo; out->trim_len = w.len; }
