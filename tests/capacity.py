@@ -26,6 +26,7 @@ DEFINES = {"FPL_NUM_SMS": "fpl_device.cuh", "CS_TILE": "fpl_stats.cu", "CS_GROUP
            "RQ_LONG": "fpl_stats.cu", "RQ_LIST": "fpl_stats.cu"}
 # kernel -> (source file, text in front of its grid-cap expression): grid = min(want, FPL_NUM_SMS * factor)
 GRID_CAPS = {"k_kmer_fix": ("fpl_stats.cu", "void launch_kmer_fix("), "k_read_qual": ("fpl_stats.cu", "void launch_read_qual("),
+             "k_read_qual_exc": ("fpl_stats.cu", "void launch_read_qual_exc("),
              "k_fastq_pack": ("fpl_ingest.cu", "k_fastq_pack<<<"), "k_emit_copy": ("fpl_emit.cu", "k_emit_copy<<<")}
 
 
@@ -68,7 +69,7 @@ def constants(texts=None):
         threads = launch.split(",")[1].strip()
         threads = threads.replace("KF_WARPS", str(out["KF_WARPS"])).replace("RQ_WARPS", str(out["RQ_WARPS"]))
         out[kern + "_WARPS"] = _value(threads) // 32
-    assert out["k_kmer_fix_WARPS"] == out["KF_WARPS"] and out["k_read_qual_WARPS"] == out["RQ_WARPS"]
+    assert out["k_kmer_fix_WARPS"] == out["KF_WARPS"] and out["k_read_qual_WARPS"] == out["k_read_qual_exc_WARPS"] == out["RQ_WARPS"]
     return out
 
 
@@ -86,12 +87,31 @@ def shrunk_sources(base=None, **values):
     return texts
 
 
+# ---- which kernels made the quality histograms and the medians ----
+# "scan": k_scan_jit counted them and k_read_qual_exc treated the reads k_final listed; "read_qual": k_read_qual did (every
+# other scan kernel, -Q -L, and the pre-filter half of --mask/--break)
+QUAL_TIMERS = {"scan": "k_read_qual(exceptions)", "read_qual": "k_read_qual(pre+post)"}
+
+
+def quality_pass(eng):
+    """"scan" or "read_qual", from the launches eng has timed: eng.set_timing(True) goes before its first process call"""
+    kt = eng.kernel_times()
+    ran = [name for name, timer in QUAL_TIMERS.items() if kt[timer][1] > 0]
+    assert len(ran) == 1, f"quality passes that ran: {ran or 'none (is timing on?)'}"
+    return ran[0]
+
+
 # ---- comparison with the oracle (records, both Stats blocks, counters, -N/-b lists) ----
-def compare_with_oracle(eng, opt, batch, what, oracle=None):
-    """eng: a fresh binding.Engine (GPU or emulated).  Returns the oracle's records."""
+def compare_with_oracle(eng, opt, batch, what, oracle=None, qual_pass=None):
+    """eng: a fresh binding.Engine (GPU or emulated).  qual_pass: the quality pass (quality_pass) that has to have run.
+    Returns the oracle's records."""
     o = oracle or OracleEngine(opt)
     exp = o.process(batch)
+    eng.set_timing(qual_pass is not None)
     compare_results(eng.process(batch), exp, what)
+    if qual_pass is not None:
+        got = quality_pass(eng)
+        assert got == qual_pass, f"{what}: expected the {qual_pass} pass, got {got}"
     if opt.mask or opt.break_reads:
         compare_lists(eng.segments(), o.segments(), what + "/segments")
         compare_lists(eng.mask_regions(), o.mask_regions(), what + "/regions")
@@ -135,6 +155,8 @@ CS_SETS = {
     "mask": Options(start_adapter=S, end_adapter=E, trimming_extension=0, trim_front=3, trim_tail=2, disable_quality_filtering=True,
                     length_required=1, mask=True, mask_window_size=5, mask_mean_quality=12),
 }
+# the quality pass each takes on the default (jit) scan: the length filter is on; --mask keeps k_read_qual
+CS_PASS = {"plain": "scan", "mask": "read_qual"}
 
 
 def cycle_counts(k):
@@ -319,6 +341,149 @@ def stride_batch(k, seed):
     lens = rng.integers(0, 121, size=n)
     lens[::97] = 600
     return pack_reads([(_bases(rng, int(L)), _quals(rng, int(L), 1, 90)) for L in lens])
+
+
+# ---- k_read_qual_exc: the list k_final makes of the reads whose one passing segment is not their window ----
+END = 240          # adapters planted in the middle stay this far from both ends of the window (outside the end-trim windows)
+EXC_KINDS = ("dead", "split", "left_fails", "right_fails", "none_pass", "gap_largest", "seg0_right", "fails", "cut_split")
+
+
+def decided_read(rng, kind, L, wide=False):
+    """one read of L bases whose segments k_final decides as `kind` under RQ_OPT (the split kinds want L >= 4 * END,
+    "cut_split" 9 * END).  wide: quality bytes over all of 1..127 between two ends of 40 good bases."""
+    s = bytearray(_bases(rng, L))
+    q = bytearray(_quals(rng, L, 20, 40))
+    if wide and L > 80:
+        q[40:L - 40] = rng.integers(1, 128, size=L - 80).astype(np.uint8).tobytes()
+    a = int(rng.integers(L // 3, max(L // 2, L // 3 + 1)))
+    if kind in ("split", "left_fails", "right_fails", "none_pass"):   # a start adapter in the middle: two parts
+        if kind == "none_pass":                  # ... which both fail the filter (N bases)
+            s[::3] = b"N" * len(s[::3])
+        s[a:a + len(S)] = S.encode()
+        if kind == "left_fails":
+            s[a // 4:a // 2] = b"N" * (a // 2 - a // 4)
+        elif kind == "right_fails":
+            b0, n = a + len(S), L - a - len(S)
+            s[b0 + n // 4:b0 + n // 2] = b"N" * (n // 2 - n // 4)
+    elif kind == "gap_largest":                  # both adapters far apart: the gap between them is the largest part
+        s[END:END + len(S)] = S.encode()
+        e = L - END - len(E)
+        s[e:e + len(E)] = E.encode()
+    elif kind == "seg0_right":                   # an end adapter within the trimming extension of the front: one, right part
+        s[4:4 + len(E)] = E.encode()
+    elif kind == "fails":                        # unsplit, the one segment fails the quality filter
+        q[:] = rng.integers(1, 61, size=L).astype(np.uint8).tobytes() if wide else _quals(rng, L, 1, 12)
+        e = min(40, L // 4)
+        q[:e] = _q(e, 30)
+        q[L - e:] = _q(e, 30)
+    elif kind == "dead":                         # the quality cut drops it
+        q[:] = rng.integers(1, 46, size=L).astype(np.uint8).tobytes() if wide else _q(L, 0)
+    elif kind == "cut_head":                     # a long low-quality head that the front cut removes
+        q[:L // 3] = _q(L // 3, 2)
+    elif kind == "cut_split":                    # the cuts leave the middle third, and that window is split 1 : 2
+        assert L >= 9 * END
+        q[:L // 3] = _q(L // 3, 2)
+        q[L - L // 3:] = _q(L // 3, 2)
+        a = L // 3 + L // 9
+        s[a:a + len(S)] = S.encode()
+    else:
+        assert kind == "plain", kind
+    return bytes(s), bytes(q)
+
+
+def listed(res):
+    """per read (on the oracle's records): k_final puts it on k_read_qual_exc's list — every read but the ones whose one
+    passing segment is the whole of their window"""
+    split = (res["flags"] & abi.FLAG_MIDDLE_ADAPTER) != 0
+    return split | (res["n_segments"] != 1) | (res["seg_result"][:, 0] != abi.PASS_FILTER)
+
+
+def check_exc_kinds(batch, res, k):
+    """the listed reads longer than RQ_LONG reach every kind of EXC_KINDS (on the oracle's records)"""
+    r = res[listed(res) & (batch.lens > k["RQ_LONG"])]
+    L = batch.lens[listed(res) & (batch.lens > k["RQ_LONG"])]
+    flags, nseg, sr = r["flags"], r["n_segments"], r["seg_result"]
+    split = (flags & abi.FLAG_MIDDLE_ADAPTER) != 0
+    ok = (sr == abi.PASS_FILTER) & (np.arange(sr.shape[1])[None, :] < nseg[:, None])
+    two = split & (nseg == 2)
+    gap = r["seg_lo"][:, 1] - (r["seg_lo"][:, 0] + r["seg_len"][:, 0])
+    # "cut_split": a window well inside the read, its smaller part counted directly and its larger one by subtraction
+    window = r["seg_lo"][:, 1] + r["seg_len"][:, 1] - r["seg_lo"][:, 0]
+    inside = two & ok.all(axis=1) & (r["seg_lo"][:, 0] > L // 4) & (window < L // 2)
+    found = {"dead": (flags & abi.FLAG_DROPPED_BY_CUT) != 0, "split": two & ok.all(axis=1), "left_fails": two & ~ok[:, 0] & ok[:, 1],
+             "right_fails": two & ok[:, 0] & ~ok[:, 1], "none_pass": two & ~ok.any(axis=1),
+             "gap_largest": two & (gap > r["seg_len"].max(axis=1)), "seg0_right": (flags & abi.FLAG_SEG0_IS_RIGHT) != 0,
+             "fails": ~split & (nseg == 1) & ~ok[:, 0],
+             "cut_split": inside & (2 * r["seg_len"][:, 0] < window) & (2 * r["seg_len"][:, 1] >= window)}
+    assert set(found) == set(EXC_KINDS)
+    for kind, m in found.items():
+        assert m.any(), f"no listed long read of kind {kind}"
+
+
+def _long_len(k, j):
+    return max(k["RQ_LONG"] + 1, 9 * END) + 37 * j
+
+
+def exc_min_overflow(k):
+    """the shortest list of long reads of which block 0 of k_read_qual_exc's capped grid meets RQ_LIST + 1, in any order"""
+    w = k["RQ_WARPS"]
+    return (k["RQ_LIST"] // w) * w * k["k_read_qual_exc_BLOCKS"] + k["RQ_LIST"] % w + 1
+
+
+def exc_overflow_batch(k, seed):
+    """every listed read is longer than RQ_LONG and the list is longer than exc_min_overflow: whatever its order, block 0
+    meets more than RQ_LIST long reads and hands the rest to lone warps.  The reads that are not listed are short, and
+    enough for the grid to reach its cap."""
+    rng = np.random.default_rng(seed)
+    n_long = exc_min_overflow(k) + 2 * len(EXC_KINDS)
+    reads = [decided_read(rng, EXC_KINDS[j % len(EXC_KINDS)], _long_len(k, j)) for j in range(n_long)]
+    reads += [decided_read(rng, "plain", int(rng.integers(50, 150))) for _ in range(k["RQ_WARPS"] * k["k_read_qual_exc_BLOCKS"] + 5)]
+    return pack_reads(_shuffled(rng, reads))
+
+
+def exc_kinds_batch(k, seed):
+    """two reads longer than RQ_LONG of every kind of EXC_KINDS, a long and some short reads that are not listed, and short
+    listed ones"""
+    rng = np.random.default_rng(seed)
+    reads = [decided_read(rng, kind, _long_len(k, j)) for j, kind in enumerate(EXC_KINDS + EXC_KINDS)]
+    reads += [decided_read(rng, kind, _long_len(k, 3)) for kind in ("plain", "cut_head")]
+    reads += [decided_read(rng, ("plain", "dead", "fails")[i % 3], int(rng.integers(50, 300))) for i in range(30)]
+    return pack_reads(_shuffled(rng, reads))
+
+
+LOOP_KINDS = ("dead", "fails", "split", "dead", "left_fails", "fails", "none_pass", "right_fails")
+
+
+def exc_loop_batch(k, seed):
+    """a list longer than k_read_qual_exc's capped grid has warps: warps loop, and each block takes many windows out of
+    the post-filter sums before its one flush.  Mostly short listed reads with quality bytes over 1..127, one long read of
+    every kind among them, and reads that are not listed."""
+    rng = np.random.default_rng(seed)
+    n = k["RQ_WARPS"] * k["k_read_qual_exc_BLOCKS"] * 9 // 8 + 11
+    reads = []
+    for i in range(n):
+        kind = LOOP_KINDS[i % len(LOOP_KINDS)]
+        L = int(rng.integers(20, 200)) if kind in ("dead", "fails") else 4 * END + int(rng.integers(0, 200))
+        reads.append(decided_read(rng, kind, L, wide=True))
+    reads += [decided_read(rng, "plain", int(rng.integers(50, 400)), wide=True) for _ in range(n // 8)]
+    reads += [decided_read(rng, kind, _long_len(k, j), wide=j % 2 == 1) for j, kind in enumerate(EXC_KINDS)]
+    return pack_reads(_shuffled(rng, reads))
+
+
+def exc_list_batch(k, seed, every):
+    """every: every read is listed (short ones of every kind, empty ones); otherwise none is (*n_exc == 0, every block of
+    k_read_qual_exc idles)"""
+    rng = np.random.default_rng(seed)
+    reads = []
+    for i in range(5 * k["RQ_WARPS"] + 3):
+        if not every:
+            reads.append(decided_read(rng, ("plain", "cut_head")[i % 2], int(rng.integers(50, 400))))
+        elif i % 10 == 9:
+            reads.append((b"", b""))
+        else:
+            kind = EXC_KINDS[i % len(EXC_KINDS)]
+            reads.append(decided_read(rng, kind, 9 * END + i if kind not in ("dead", "fails") else 30 + i))
+    return pack_reads(reads)
 
 
 # ---- the FASTQ text path: more records than k_fastq_pack and k_emit_copy have warps ----

@@ -7,6 +7,9 @@ those paths, next to reads that trimAndCut drops, and compare records, both Stat
     the right side), and whose left part fails the filter;
   - long and short reads dropped by the quality cut in the same block as the long list;
   - the same batch under --mask/--break, where k_read_qual counts the pre-filter Stats only.
+k_read_qual makes the post-filter histograms where k_scan_jit does not count them: the cases run with FPL_NO_JIT=1
+(k_scan_fast) for that, and on the default scan too, where k_read_qual_exc treats the same reads from k_final's list (in
+the list's order: the placement below means nothing there).  Every case asserts which of the two ran.
 
 Runs on the GPU and, with FPL_EMULATE=1, on the emulated library (tests/test_capacity_shrunk_long_reads.py runs the same
 cases on the shrunk build)."""
@@ -23,33 +26,12 @@ S, E = capacity.S, capacity.E
 OPT = Options(start_adapter=S, end_adapter=E, cut_front=True, cut_tail=True, length_required=1)
 EXT_OPT = cases.MASK_BREAK_SETS["mask_and_break"]
 KINDS = ("split", "gap_largest", "seg0_right", "left_fails", "dead", "plain")
-END = 240          # adapters planted in the middle stay this far from both read ends (outside the end-trim windows)
-
-
-def _long_read(rng, kind, L):
-    s = bytearray(capacity._bases(rng, L))
-    q = bytearray(capacity._quals(rng, L, 20, 40))
-    if kind == "split":                      # a start adapter in the middle: two passing parts
-        a = int(rng.integers(L // 3, L // 2))
-        s[a:a + len(S)] = S.encode()
-    elif kind == "gap_largest":              # both adapters far apart: the gap between them is the largest part
-        s[END:END + len(S)] = S.encode()
-        e = L - END - len(E)
-        s[e:e + len(E)] = E.encode()
-    elif kind == "seg0_right":               # an end adapter within the trimming extension of the front: one, right part
-        s[4:4 + len(E)] = E.encode()
-    elif kind == "left_fails":               # a split read whose left part fails the filter (20 % N bases)
-        a = int(rng.integers(L // 3, L // 2))
-        s[a:a + len(S)] = S.encode()
-        s[a // 4:a // 4 + a // 5] = b"N" * (a // 5)
-    elif kind == "dead":                     # the quality cut drops it
-        q[:] = capacity._q(L, 0)
-    return bytes(s), bytes(q)
+END = capacity.END
 
 
 def long_decision_batch(k, seed):
-    """RQ_LIST + 1 long reads at the indices block 0 visits (the last one goes to a lone warp) and len(KINDS) at block 1's,
-    cycling through KINDS; every other read short: dropped by the cut, empty, or one base"""
+    """RQ_LIST + 1 long reads at the indices block 0 of k_read_qual visits (the last one goes to a lone warp) and len(KINDS)
+    at block 1's, cycling through KINDS; every other read short: dropped by the cut, empty, or one base"""
     rng = np.random.default_rng(seed)
     at = capacity.rq_indices(k, 0, k["RQ_LIST"] + 1) + capacity.rq_indices(k, 1, len(KINDS))
     n = max(at) + 1 + 5
@@ -62,7 +44,7 @@ def long_decision_batch(k, seed):
             reads.append(((b"", b""), (b"A", b"5"))[i % 3 - 1])
     for j, i in enumerate(at):
         L = max(k["RQ_LONG"] + 1, 4 * END) + 37 * j
-        reads[i] = _long_read(rng, KINDS[j % len(KINDS)], L)
+        reads[i] = capacity.decided_read(rng, KINDS[j % len(KINDS)], L)
     return pack_reads(reads), at
 
 
@@ -80,16 +62,18 @@ def check_shapes(batch, at, res):
     assert ((two["seg_result"][:, 0] != abi.PASS_FILTER) & (two["seg_result"][:, 1] == abi.PASS_FILTER)).any()
 
 
-def run_cases(make_engine, k, what):
+def run_cases(make_engine, scans, k, what):
+    """make_engine(opt, scan); scans: {scan: the quality pass OPT takes with it}"""
     batch, at = long_decision_batch(k, 11)
-    res = capacity.compare_with_oracle(make_engine(OPT), OPT, batch, f"{what}/decisions")
-    check_shapes(batch, at, res)
-    # short reads dropped by the cut share block 0 with the long list
-    dropped = np.flatnonzero(res["flags"] & abi.FLAG_DROPPED_BY_CUT)
-    assert (dropped < k["RQ_WARPS"]).any() and (batch.lens[dropped] <= k["RQ_LONG"]).any()
-    capacity.compare_with_oracle(make_engine(EXT_OPT), EXT_OPT, batch, f"{what}/mask_break")
+    for scan, qual_pass in scans.items():
+        res = capacity.compare_with_oracle(make_engine(OPT, scan), OPT, batch, f"{what}/decisions/{scan}", qual_pass=qual_pass)
+        check_shapes(batch, at, res)
+        # short reads dropped by the cut share block 0 with the long list
+        dropped = np.flatnonzero(res["flags"] & abi.FLAG_DROPPED_BY_CUT)
+        assert (dropped < k["RQ_WARPS"]).any() and (batch.lens[dropped] <= k["RQ_LONG"]).any()
+        capacity.compare_with_oracle(make_engine(EXT_OPT, scan), EXT_OPT, batch, f"{what}/mask_break/{scan}", qual_pass="read_qual")
 
 
 def test_long_read_decisions():
-    from fastplong_b200.binding import Engine
-    run_cases(Engine, capacity.constants(), "gpu")
+    from test_gpu_capacity import SCANS, engine
+    run_cases(engine, {scan: qual_pass for scan, (_, qual_pass) in SCANS.items()}, capacity.constants(), "gpu")

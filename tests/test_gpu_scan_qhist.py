@@ -7,8 +7,9 @@ cut, split (with zero, one or two passing parts), or with a failing segment — 
 k_read_qual_exc takes its window out of the post-filter sums and counts it the way k_read_qual does.  k_count adds the
 per-read sums.  These batches put reads of every exception kind through that path (next to ordinary ones, including
 reads past RQ_LONG, which k_read_qual_exc streams block-wide) and compare records, both Stats blocks and the counters
-with the oracle; the kernel times say which path ran.  FPL_NO_JIT=1 runs the same cases on k_scan_fast, which keeps
-k_read_qual.
+with the oracle; the kernel times say which path ran (capacity.quality_pass).  FPL_NO_JIT=1 runs the same cases on
+k_scan_fast, which keeps k_read_qual.  One submission also runs in several tiles (read tiling of a device batch, upload
+pieces of a host batch): the exception list restarts per tile and the striped sums are folded once per call.
 
 Runs on the GPU and, with FPL_EMULATE=1, on the emulated library."""
 import numpy as np
@@ -26,38 +27,17 @@ OPT = Options(start_adapter=S, end_adapter=E, cut_front=True, cut_tail=True, len
 # -Q -L: the scan has no filter counts to take, loads no quality bytes and leaves the histograms to k_read_qual
 OPT_QL = Options(start_adapter=S, end_adapter=E, disable_quality_filtering=True, disable_length_filtering=True)
 SCANS = {"jit": {}, "no_jit": {"FPL_NO_JIT": "1"}}
-EXC, FULL = "k_read_qual(exceptions)", "k_read_qual(pre+post)"
 
 
 def _read(rng, kind, L):
     """one read of an exception kind (or an ordinary one: "plain")"""
-    s = bytearray(capacity._bases(rng, L))
-    q = bytearray(capacity._quals(rng, L, 20, 40))
-    a = L // 2
-    if kind == "split2":                         # a start adapter in the middle: two passing parts
-        s[a:a + len(S)] = S.encode()
-    elif kind == "split1":                       # ... whose left part fails the filter (N bases)
-        s[a:a + len(S)] = S.encode()
-        s[a // 4:a // 4 + a // 4] = b"N" * (a // 4)
-    elif kind == "split0":                       # ... whose two parts both fail
-        s[a:a + len(S)] = S.encode()
-        s[:] = bytes(b if i % 3 else ord("N") for i, b in enumerate(s))
-        s[a:a + len(S)] = S.encode()
-    elif kind == "fails":                        # unsplit, the one segment fails the quality filter
-        q[:] = capacity._quals(rng, L, 1, 12)
-        q[:40] = capacity._q(40, 30)
-        q[-40:] = capacity._q(40, 30)
-    elif kind == "dead":                         # the quality cut drops it
-        q[:] = capacity._q(L, 0)
-    elif kind == "cut_head":                     # a long low-quality head that the front cut removes
-        h = L // 3
-        q[:h] = capacity._q(h, 2)
-    elif kind == "short_fails":                  # passes everything but the length filter
-        s, q = s[:30], q[:30]
-    return bytes(s), bytes(q)
+    if kind == "short_fails":                    # passes everything but the length filter
+        s, q = capacity.decided_read(rng, "plain", L)
+        return s[:30], q[:30]
+    return capacity.decided_read(rng, kind, L)
 
 
-KINDS = ("plain", "split2", "split1", "split0", "fails", "dead", "cut_head", "short_fails")
+KINDS = ("plain", "split", "left_fails", "none_pass", "fails", "dead", "cut_head", "short_fails")
 
 
 def exception_batch(seed, n=160, long_reads=True):
@@ -69,14 +49,14 @@ def exception_batch(seed, n=160, long_reads=True):
     reads += [(b"", b""), (b"A", b"5"), (b"C", b"#"), (b"", b"")]
     if long_reads:
         rq_long = capacity.constants()["RQ_LONG"]
-        for j, kind in enumerate(("plain", "split2", "split1", "dead", "cut_head")):
+        for j, kind in enumerate(("plain", "split", "left_fails", "dead", "cut_head")):
             reads.insert(7 * j + 3, _read(rng, kind, rq_long + 1 + 101 * j))
     return pack_reads(reads)
 
 
 def make_engine(opt, env, monkeypatch):
     from fastplong_b200.binding import Engine
-    for k in ("FPL_NO_JIT",):
+    for k in ("FPL_NO_JIT", "FPL_TILE_MBASES", "FPL_PIECE_MB"):
         monkeypatch.delenv(k, raising=False)
     for k, v in env.items():
         monkeypatch.setenv(k, v)
@@ -86,12 +66,9 @@ def make_engine(opt, env, monkeypatch):
 
 
 def check_path(g, scan, opt):
-    kt = g.kernel_times()
     counts = not (opt.disable_quality_filtering and opt.disable_length_filtering)
-    if scan == "jit" and counts and not (opt.mask or opt.break_reads):
-        assert kt[EXC][1] > 0 and kt[FULL][1] == 0, kt
-    else:
-        assert kt[EXC][1] == 0 and kt[FULL][1] > 0, kt
+    expected = "scan" if scan == "jit" and counts and not (opt.mask or opt.break_reads) else "read_qual"
+    assert capacity.quality_pass(g) == expected, g.kernel_times()
 
 
 def run(opt, batches, scan, what, monkeypatch):
@@ -146,3 +123,35 @@ def test_several_calls(scan, monkeypatch):
 def test_quality_domain(name, scan, monkeypatch):
     """quality bytes over 1..127 with the quality options at their ends (the --mask / --break sets keep k_read_qual)"""
     run(cases.QUALITY_SETS[name], [cases.quality_domain_batch(5)], scan, f"{name}/{scan}", monkeypatch)
+
+
+@pytest.mark.parametrize("how", ["tiles", "pieces"])
+def test_one_submission_in_several_tiles(how, monkeypatch):
+    """one call whose reads run tile by tile — FPL_TILE_MBASES=1 on a device batch, 1 MiB upload pieces of a host batch: the
+    exception list restarts and moves on with each tile, the stripes are indexed by the tile's read numbers, one fold"""
+    import layouts
+    from test_gpu_layout import device_buffers
+    b = exception_batch(4, n=2400)
+    assert b.n_bases > 4000000
+    g = make_engine(OPT, {"tiles": {"FPL_TILE_MBASES": "1"}, "pieces": {"FPL_PIECE_MB": "1"}}[how], monkeypatch)
+    o = OracleEngine(OPT)
+    try:
+        if how == "tiles":
+            relaid = layouts.relayout(b, tail=64)
+            n_bytes = layouts.end_of_reads(relaid)
+            bufs = device_buffers(relaid, n_bytes)
+            g.process_device(*(x.data_ptr() for x in bufs), b.n_reads, n_bytes)
+            g.sync()
+            res = g.fetch_results(b.n_reads)
+        else:
+            res = g.process(b)
+        compare_results(res, o.process(b), how)
+        cyc = int(b.lens.max())
+        for w in (0, 1):
+            compare_stats(g.stats(w, cyc), o.stats(w, cyc), f"{how}/stats{w}")
+        compare_stats(g.counters(), o.counters(), how + "/counters")
+        check_path(g, "jit", OPT)
+        kt = g.kernel_times()
+        assert kt[capacity.QUAL_TIMERS["scan"]][1] >= 3 and kt["k_qhist_fold"][1] == 1, kt
+    finally:
+        g.close()

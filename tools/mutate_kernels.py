@@ -41,6 +41,7 @@ def battery(lib, small=None):
                 CS.test_cycle_stats_post_filter_counts(SHRUNK, optset)
             CS.test_kmer_fix_long_range_list(SHRUNK)
             CS.test_read_qual_long_list_and_stride(SHRUNK)
+            CS.test_read_qual_exc_list(SHRUNK)
             CS.test_text_path_more_records_than_warps(SHRUNK)
         T.check(capacity.HEADROOM_OPT, capacity.headroom_batch(capacity.constants(), False), "packed counter at its fullest")
         for name, (opt, b) in cases.edge_cases().items():
