@@ -2,7 +2,7 @@
 import ctypes as C
 import numpy as np
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 COMM_ID_BYTES = 128        # FPL_COMM_ID_BYTES == sizeof(ncclUniqueId)
 MAX_ADAPTER_LEN = 1024
 MAX_ADAPTERS = 1024
@@ -75,6 +75,12 @@ class FplOutBatch(C.Structure):
 class FplReportInfo(C.Structure):
     """fpl_report_info: what fpl_report_json takes beyond the context's Options"""
     _fields_ = [("struct_size", C.c_int32), ("is_rna", C.c_int32), ("version", C.c_char_p), ("command", C.c_char_p)]
+
+
+class FplReportHtmlInfo(C.Structure):
+    """fpl_report_html_info: what fpl_report_html takes beyond the context's Options and read lists"""
+    _fields_ = [("struct_size", C.c_int32), ("is_rna", C.c_int32), ("version", C.c_char_p), ("command", C.c_char_p),
+                ("title", C.c_char_p), ("time_text", C.c_char_p)]
 
 
 RESULT_DTYPE = np.dtype([

@@ -6,7 +6,7 @@ import os
 import numpy as np
 
 from . import abi
-from .abi import FplAdapters, FplBatch, FplOptions, FplOutBatch, FplReportInfo, RESULT_DTYPE
+from .abi import FplAdapters, FplBatch, FplOptions, FplOutBatch, FplReportHtmlInfo, FplReportInfo, RESULT_DTYPE
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libfplgpu.so")
@@ -64,6 +64,8 @@ def load_library():
     lib.fpl_eval_pick_adapter.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_char_p, C.c_int32]
     lib.fpl_reset.argtypes = [C.c_void_p]
     lib.fpl_report_json.argtypes = [C.c_void_p, C.POINTER(FplReportInfo), C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
+    lib.fpl_keep_read_lists.argtypes = [C.c_void_p, C.c_int]
+    lib.fpl_report_html.argtypes = [C.c_void_p, C.POINTER(FplReportHtmlInfo), C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
     lib.fpl_last_kernel_times.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(C.c_float),
                                           C.POINTER(C.c_int64), C.c_int]
     lib.fpl_launch_count.argtypes = [C.c_void_p]
@@ -80,7 +82,7 @@ EXPORTS = ["fpl_last_error", "fpl_abi_version", "fpl_create", "fpl_destroy", "fp
            "fpl_sync", "fpl_stream", "fpl_last_segments", "fpl_last_mask_regions", "fpl_fetch_results", "fpl_stats_cycles", "fpl_stats_reserve", "fpl_stats_download",
            "fpl_stats_device_ptr", "fpl_counter_words", "fpl_counters_download", "fpl_counters_device_ptr",
            "fpl_comm_unique_id", "fpl_comm_init", "fpl_comm_destroy", "fpl_comm_size", "fpl_comm_agree_cycles", "fpl_allreduce_stats",
-           "fpl_eval_adapter_kmers", "fpl_eval_pick_adapter", "fpl_report_json", "fpl_reset", "fpl_last_kernel_times", "fpl_launch_count", "fpl_set_timing"]
+           "fpl_eval_adapter_kmers", "fpl_eval_pick_adapter", "fpl_report_json", "fpl_keep_read_lists", "fpl_report_html", "fpl_reset", "fpl_last_kernel_times", "fpl_launch_count", "fpl_set_timing"]
 
 
 class _DeviceArray:
@@ -288,6 +290,28 @@ class Engine:
             self._check(rc)
         buf = np.empty(n.value, dtype=np.uint8)
         self._check(self.lib.fpl_report_json(self.h, C.byref(info), buf.ctypes.data, buf.size, C.byref(n)))
+        return buf.tobytes()
+
+    def keep_read_lists(self, on=True):
+        """Keep the per-read (length, median quality) lists of both Stats blocks on the device from the next process*() call
+        on (fpl_keep_read_lists); report_html() needs them for every call since the engine was made or reset."""
+        self._check(self.lib.fpl_keep_read_lists(self.h, int(bool(on))))
+
+    def report_html(self, command="", version="0.4.1", title="fastplong report", time_text=None, is_rna=False):
+        """fastplong's HTML report (-h) of the accumulators and read lists, byte for byte as HtmlReporter::report writes it at
+        -w 1 (fpl_report_html).  time_text None: the local time as the reference formats it."""
+        if time_text is None:
+            import time
+            t = time.localtime()
+            time_text = "%d-%02d-%02d      %02d:%02d:%02d" % (t.tm_year, t.tm_mon, t.tm_mday, t.tm_hour, t.tm_min, t.tm_sec)
+        info = FplReportHtmlInfo(C.sizeof(FplReportHtmlInfo), int(bool(is_rna)), version.encode(), command.encode(), title.encode(),
+                                 time_text.encode())
+        n = C.c_int64()
+        rc = self.lib.fpl_report_html(self.h, C.byref(info), None, 0, C.byref(n))
+        if rc < 0:
+            self._check(rc)
+        buf = np.empty(n.value, dtype=np.uint8)
+        self._check(self.lib.fpl_report_html(self.h, C.byref(info), buf.ctypes.data, buf.size, C.byref(n)))
         return buf.tobytes()
 
     # --- multi-GPU merge (one process per GPU): Stats::merge / FilterResult::merge as NCCL all-reduces ---

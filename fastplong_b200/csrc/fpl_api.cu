@@ -49,6 +49,18 @@ void launch_make_preseg(const DevBatch&, StatSeg*, cudaStream_t);
 void launch_report_cycles(const unsigned long long*, const unsigned long long*, int64_t, unsigned long long*, cudaStream_t);
 void launch_report_sizes(const ReportCurves&, int64_t*, cudaStream_t);
 void launch_report_text(const ReportCurves&, const int64_t*, const uint8_t*, const int64_t*, const int64_t*, int, uint8_t*, cudaStream_t);
+void launch_html_capture(const fpl_read_result*, const int32_t*, int64_t, const fpl_segment*, int64_t, HtmlEntry*, HtmlEntry*, cudaStream_t);
+void launch_html_hist(const HtmlEntry*, int64_t, int64_t, long long*, cudaStream_t);
+void launch_html_scatter(const HtmlEntry*, int64_t, int64_t, const long long*, HtmlEntry*, cudaStream_t);
+void launch_html_lenhist(const HtmlEntry*, int64_t, unsigned long long*, cudaStream_t);
+void launch_html_lenprod(const unsigned long long*, int64_t, long long*, cudaStream_t);
+void launch_html_lensearch(const unsigned long long*, const long long*, const long long*, const long long*, int64_t, long long,
+                           unsigned long long, int*, cudaStream_t);
+void launch_html_bins(const unsigned long long*, int64_t, int64_t, unsigned long long*, cudaStream_t);
+void launch_html_values(const unsigned long long*, int64_t, int64_t, int, double*, cudaStream_t);
+void launch_html_sums(const double*, int64_t, const long long*, int64_t, double*, cudaStream_t);
+void launch_html_sizes(const HtmlText&, int64_t*, cudaStream_t);
+void launch_html_text(const HtmlText&, const int64_t*, const uint8_t*, const int64_t*, const int64_t*, int, uint8_t*, cudaStream_t);
 
 static thread_local char g_err[512] = "";
 
@@ -67,7 +79,9 @@ static int fail(const char* fmt, ...) {
     } while (0)
 
 enum { K_PRESEG, K_CYCLE_PRE, K_QUAL_PRE, K_TRIM, K_SCAN, K_FINAL, K_COUNT, K_CYCLE_POST, K_QUAL_POST, K_KMER_FIX, K_ALLREDUCE,
-       K_EMIT_BATCH_SIZES, K_EMIT_BATCH_COPY, K_REPORT_CYCLES, K_REPORT_SIZES, K_REPORT_TEXT, K_QUAL_EXC, K_QHIST_FOLD, K_NKERNELS };
+       K_EMIT_BATCH_SIZES, K_EMIT_BATCH_COPY, K_REPORT_CYCLES, K_REPORT_SIZES, K_REPORT_TEXT, K_QUAL_EXC, K_QHIST_FOLD,
+       K_HTML_CAPTURE, K_HTML_CYCLES, K_HTML_GROUP_HIST, K_HTML_GROUP_SCATTER, K_HTML_LENGTHS, K_HTML_VALUES, K_HTML_SUMS,
+       K_HTML_SIZES, K_HTML_TEXT, K_NKERNELS };
 // K_CYCLE_PRE: the fused pass (both Stats blocks) without --mask/--break, the pre-filter pass with it; K_CYCLE_POST: the
 // post-filter segments the fused pass did not take, or the whole --mask/--break post-filter list.  K_QUAL_EXC and
 // K_QHIST_FOLD replace K_QUAL_PRE where k_scan_jit counts the quality histograms.
@@ -76,7 +90,43 @@ static const char* const kKernelNames[K_NKERNELS] = {"k_make_preseg", "k_cycle_s
                                                      "k_cycle_stats(post residual)", "k_read_qual(post)", "k_kmer_fix",
                                                      "nccl_allreduce(stats)", "k_emit_batch(sizes)", "k_emit_batch(copy)",
                                                      "k_report(cycles)", "k_report(sizes)", "k_report(text)",
-                                                     "k_read_qual(exceptions)", "k_qhist_fold"};
+                                                     "k_read_qual(exceptions)", "k_qhist_fold",
+                                                     "k_html(capture)", "k_html(cycles)", "k_html(group hist)", "k_html(group scatter)",
+                                                     "k_html(lengths)", "k_html(values)", "k_html(sums)", "k_html(sizes)",
+                                                     "k_html(text)"};
+// K_HTML_CYCLES: k_report_cycles + k_html_bins; K_HTML_LENGTHS: k_html_lenhist, k_html_lenprod, k_html_lensearch
+
+// fpl_keep_read_lists: the (length, median) lists of both Stats blocks
+struct FplLists {
+    HtmlEntry* d[2] = {nullptr, nullptr};
+    int64_t cap[2] = {0, 0}, n[2] = {0, 0};
+    bool keep = false;                  // capture on
+    bool complete = true;               // every fpl_process_* call since fpl_create / fpl_reset captured
+    bool merged = false;                // fpl_allreduce_stats over more than one rank since then
+};
+
+// fpl_report_html: the text and its work buffers
+struct FplHtml {
+    HtmlEntry* d_grp[2] = {nullptr, nullptr}; int64_t cap_grp[2] = {0, 0};
+    long long* d_mat = nullptr; int64_t cap_mat = 0;     // grouping histograms, then their exclusive sum in place
+    long long* d_moff = nullptr; int64_t cap_moff = 0;
+    unsigned long long* d_hist = nullptr; int64_t cap_hist = 0;   // length histogram
+    long long* d_lwork = nullptr; int64_t cap_lwork = 0;          // count scan, products, product scan
+    int* d_lstat = nullptr;                                       // min, max, median, N50 of each block
+    unsigned long long* d_sum = nullptr;                          // k_report_cycles' 6 words, then 16 base-bin counts
+    long long* d_x = nullptr; int64_t cap_x = 0;
+    double* d_vals = nullptr; int64_t cap_vals = 0;
+    double* d_sums = nullptr; int64_t cap_sums = 0;
+    int64_t* d_size = nullptr; int64_t cap_size = 0;
+    int64_t* d_off = nullptr; int64_t cap_off = 0;
+    void* d_tmp = nullptr; int64_t cap_tmp = 0;
+    uint8_t* d_frame = nullptr; int64_t cap_frame = 0;
+    uint8_t* d_text = nullptr; int64_t cap_text = 0;
+    std::vector<uint8_t> h_frame;
+    bool built = false;
+    std::string key;
+    int64_t n_bytes = 0;
+};
 
 // fpl_report_json: the report text of the accumulators as they were when it was built, kept in HBM until a call changes them
 struct FplReport {
@@ -111,6 +161,8 @@ struct fpl_ctx {
     int n_adapters = 0;
     std::vector<std::string> adapter_str;   // fpl_adapters order (the report's adapter names and counted substrings)
     FplReport rep;
+    FplLists lists;
+    FplHtml html;
     uint8_t* d_adapters = nullptr;
     int* d_alen = nullptr;
     uint4* d_peq = nullptr;
@@ -186,7 +238,7 @@ static int ensure_reads(fpl_ctx* c, int64_t n) {
 
 static int reserve_cycles(fpl_ctx* c, int64_t need) {
     if (need <= c->C) return 0;
-    c->rep.built = false;
+    c->rep.built = false; c->html.built = false;
     int64_t nc = c->C ? c->C : 1024;
     while (nc < need) nc *= 2;
     for (int w = 0; w < 2; w++) {
@@ -205,6 +257,23 @@ static int reserve_cycles(fpl_ctx* c, int64_t need) {
         c->d_stats[w] = nb;
     }
     c->C = nc;
+    return 0;
+}
+
+// list w holds at least `need` entries, its entries kept.  Geometric, so the wait for the copy (cudaFree) is rare.
+static int grow_list(fpl_ctx* c, int w, int64_t need) {
+    FplLists& L = c->lists;
+    if (need <= L.cap[w]) return 0;
+    int64_t cap = L.cap[w] ? L.cap[w] : (1 << 16);
+    while (cap < need) cap *= 2;
+    HtmlEntry* p = nullptr;
+    CK(cudaMalloc(&p, sizeof(HtmlEntry) * cap));
+    if (L.n[w]) CK(cudaMemcpyAsync(p, L.d[w], sizeof(HtmlEntry) * L.n[w], cudaMemcpyDeviceToDevice, c->stream));
+    if (L.d[w]) {
+        CK(cudaStreamSynchronize(c->stream));
+        cudaFree(L.d[w]);
+    }
+    L.d[w] = p; L.cap[w] = cap;
     return 0;
 }
 
@@ -266,7 +335,7 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
     collect_times(c);
     c->emit_valid = false; c->emit.built = false;
     c->bemit_valid = false; c->bemit.built = false;
-    c->rep.built = false;
+    c->rep.built = false; c->html.built = false;
     c->bsrc = full;
     c->last_n = n;
     if (ensure_reads(c, n)) return -1;
@@ -375,6 +444,22 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
         r0 = r1;
     }
     if (qhist && n > 0) { Timed t(c, K_QHIST_FOLD); launch_qhist_fold(c->d_qstripes, QH_STRIPES, c->d_stats[0], c->d_stats[1], c->C, c->stream); }
+    if (c->lists.keep) {
+        // after every kernel that writes a median: the call's entries behind the lists' ends.  Without --mask/--break the
+        // post-filter list takes two slots per read (their segments), with them one per output read (ext.n_segs)
+        FplLists& L = c->lists;
+        const int64_t n_post = ext ? c->ext.n_segs : 2 * n;
+        if (grow_list(c, 0, L.n[0] + n) || grow_list(c, 1, L.n[1] + n_post)) return -1;
+        if (n || n_post) {
+            Timed t(c, K_HTML_CAPTURE);
+            launch_html_capture(d_res, full.lens, n, ext ? c->ext.d_segs : nullptr, ext ? n_post : 0, L.d[0] + L.n[0], L.d[1] + L.n[1],
+                                c->stream);
+        }
+        L.n[0] += n; L.n[1] += n_post;
+        c->html.built = false;
+    } else {
+        c->lists.complete = false;
+    }
     CK(cudaGetLastError());
     return 0;
 }
@@ -595,6 +680,13 @@ void fpl_destroy(fpl_ctx* c) {
     fpl_emit_batch_free(&c->bemit);
     cudaFree(c->rep.d_sum); cudaFree(c->rep.d_size); cudaFree(c->rep.d_off); cudaFree(c->rep.d_tmp); cudaFree(c->rep.d_frame);
     cudaFree(c->rep.d_text);
+    {
+        FplHtml& h = c->html;
+        for (int w = 0; w < 2; w++) { cudaFree(c->lists.d[w]); cudaFree(h.d_grp[w]); }
+        cudaFree(h.d_mat); cudaFree(h.d_moff); cudaFree(h.d_hist); cudaFree(h.d_lwork); cudaFree(h.d_lstat); cudaFree(h.d_sum);
+        cudaFree(h.d_x); cudaFree(h.d_vals); cudaFree(h.d_sums); cudaFree(h.d_size); cudaFree(h.d_off); cudaFree(h.d_tmp);
+        cudaFree(h.d_frame); cudaFree(h.d_text);
+    }
     if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
@@ -946,7 +1038,9 @@ int fpl_reset(fpl_ctx* c) {
         CK(cudaMemsetAsync(c->d_stats[w], 0, sizeof(unsigned long long) * FPL_STATS_WORDS(c->C), c->stream));
     CK(cudaMemsetAsync(c->d_counters, 0, sizeof(unsigned long long) * c->counter_words, c->stream));
     c->used_cycles = 0;
-    c->rep.built = false;
+    c->rep.built = false; c->html.built = false;
+    c->lists.n[0] = c->lists.n[1] = 0;
+    c->lists.complete = true; c->lists.merged = false;
     return 0;
 }
 
@@ -1081,7 +1175,8 @@ int fpl_allreduce_stats(fpl_ctx* c, int64_t cycles) {
                                              (long long)cycles, (long long)c->used_cycles);
     // rows [b*C, b*C + cycles) of the 16 per-cycle arrays, then the tail; the row pointers depend on this rank's C, the
     // counts do not, so ranks need not share a capacity.  One group = one fused launch.
-    c->rep.built = false;
+    c->rep.built = false; c->html.built = false;
+    if (c->comm_size > 1) c->lists.merged = true;
     Timed t(c, K_ALLREDUCE, false);
     CKN(nccl().GroupStart());
     for (int w = 0; w < 2; w++) {
@@ -1355,6 +1450,578 @@ extern "C" int fpl_report_json(fpl_ctx* c, const fpl_report_info* info, uint8_t*
     *n_bytes = c->rep.n_bytes;
     if (!out || cap < c->rep.n_bytes) return 1;     // the text stays built: call again with room
     CK(cudaMemcpyAsync(out, c->rep.d_text, (size_t)c->rep.n_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    collect_times(c);
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// fpl_report_html: HtmlReporter::report (src/htmlreporter.cpp:75-253) from the device accumulators and read lists.  The host
+// builds the frame — everything O(1), O(128), O(1024) or O(log total_cycles) — with the reference's own expressions; the
+// kernels of fpl_stats.cu print the density lists and the down-sampled curves into the same device buffer, between its pieces.
+// ------------------------------------------------------------------------------------------------------------------
+namespace {
+
+std::string to_str(double v) { return std::to_string(v); }        // to_string(double): "%f"
+
+std::string format_number(long number) {                          // HtmlReporter::formatNumber
+    double num = (double)number;
+    const std::string unit[6] = {"", "K", "M", "G", "T", "P"};
+    int order = 0;
+    while (num > 1000.0) {
+        order += 1;
+        num /= 1000.0;
+    }
+    if (order == 0) return std::to_string(number);
+    return std::to_string(num) + " " + unit[order];
+}
+
+std::string get_percents(long numerator, long denominator) {       // HtmlReporter::getPercents
+    if (denominator == 0) return "0.0";
+    return std::to_string((double)numerator * 100.0 / (double)denominator);
+}
+
+std::string row(const std::string& key, const std::string& v) {
+    return "<tr><td class='col1'>" + key + "</td><td class='col2'>" + v + "</td></tr>\n";
+}
+
+std::string replace_all(std::string s, const std::string& a, const std::string& b) {
+    for (size_t p = s.find(a); p != std::string::npos; p = s.find(a, p + b.size())) s.replace(p, a.size(), b);
+    return s;
+}
+
+struct HtmlBlock {                     // the merged Stats' scalars the frame prints
+    long reads, bases, lensum, cycles;
+    long base_contents[8];
+    int min_len, max_len, median_len, n50_len;
+    const long long* tail;
+    std::vector<long long> x;          // the curves' x list
+};
+
+std::vector<long long> curve_x(long cycles) {   // Stats::reportHtmlQuality / reportHtmlContents
+    std::vector<long long> x;
+    if (cycles <= 300) {
+        for (int i = 0; i < cycles; i++) x.push_back(i + 1);
+        return x;
+    }
+    for (int i = 0; i < 40 && i < cycles; i++) x.push_back(i + 1);
+    double pos = 40;
+    while (true) {
+        pos *= 1.05;
+        if (pos >= cycles) break;
+        x.push_back((int)pos);
+    }
+    if (x.back() != cycles) x.push_back(cycles);
+    return x;
+}
+
+std::string join_long(const std::vector<long long>& v) {
+    std::string s;
+    for (size_t i = 0; i < v.size(); i++) { if (i) s += ","; s += std::to_string(v[i]); }
+    return s;
+}
+
+std::string gjoin(const std::vector<double>& v) {
+    std::string s;
+    for (size_t i = 0; i < v.size(); i++) { if (i) s += ","; s += gfmt(v[i]); }
+    return s;
+}
+
+void basic_info(std::string& s, const std::string& type, const HtmlBlock& b) {   // Stats::reportHtmlBasicInfo
+    const long* bc = b.base_contents;
+    const long long* qh = b.tail + FPL_STATS_QUALHIST;
+    long q[7];                         // Q40, Q30, Q20, Q15, Q10, Q7, Q5 as Stats::summarize adds them
+    long acc = 0;
+    for (int c = 40; c < 127 - 33; c++) acc += qh[c + 33];
+    q[0] = acc;
+    const int lo[6] = {30, 20, 15, 10, 7, 5}, hi[6] = {40, 30, 20, 15, 10, 7};
+    for (int k = 0; k < 6; k++) {
+        for (int c = lo[k]; c < hi[k]; c++) acc += qh[c + 33];
+        q[k + 1] = acc;
+    }
+    const long gc = bc['G' & 7] + bc['C' & 7];
+    s += "<div class='subsection_title'>" + type + ": Basic statistics</div>\n";
+    s += "<table>\n";
+    s += row("total reads:", format_number(b.reads));
+    s += row("total bases:", format_number(b.bases));
+    s += row("minimum length:", format_number(b.min_len));
+    s += row("maximum length:", format_number(b.max_len));
+    s += row("median length:", format_number(b.median_len));
+    s += row("mean length:", format_number(b.reads == 0 ? 0 : (int)(b.lensum / b.reads)));
+    s += row("N50 length:", format_number(b.n50_len));
+    s += row("GC content:", get_percents(gc, b.bases) + "%");
+    const char* names[7] = {"Q5", "Q7", "Q10", "Q15", "Q20", "Q30", "Q40"};
+    for (int k = 0; k < 7; k++) {
+        const long v = q[6 - k];
+        s += row(std::string(names[k]) + " bases:", format_number(v) + " (" + get_percents(v, b.bases) + "%)");
+    }
+    s += "</table>\n";
+}
+
+void median_hist(std::string& s, const std::string& type, const HtmlBlock& b) {   // Stats::reporHtmlMedianQualHist
+    const std::string sub = type + ": Read median quality statistics", div = replace_all(sub, " ", "_");
+    const long long* hist = b.tail + FPL_STATS_MEDHIST;
+    const long long* bases = b.tail + FPL_STATS_MEDBASES;
+    s += "<div class='subsection_title'>" + sub + "</div>\n";
+    int minVal = 0, maxVal = 0;
+    for (int i = 0; i < 127 - 33; i++) {
+        if (bases[i + 33] == 0) minVal++;
+        else break;
+    }
+    for (int i = 127 - 33; i >= 0; i--)
+        if (bases[i + 33] > 0) { maxVal = i; break; }
+    const int offset = std::max(0, minVal - 1);
+    int total = std::min(127 - 33, maxVal - minVal + 2);
+    total = std::max(0, total);
+    std::vector<long long> x(total);
+    std::vector<double> pr(total), pb(total);
+    for (int i = 0; i < total; i++) {
+        x[i] = i + offset;
+        pr[i] = (double)hist[i + offset + 33] * 100.0 / (double)b.reads;
+        pb[i] = (double)bases[i + offset + 33] * 100.0 / (double)b.bases;
+    }
+    s += "<div id='mean_qual_length_histogram_figure'>\n";
+    s += "<div class='figure' id='plot_median_qual_hist_" + div + "' style='height:400px;'></div>\n";
+    s += "</div>\n";
+    s += "\n<script type=\"text/javascript\">\n";
+    s += "var readNum={x:[" + join_long(x) + "],y:[" + gjoin(pr) + "],name: '% reads',type:'bar',line:{color:'rgba(128,0,128,1.0)', width:1}\n};\n";
+    s += "var baseNum={x:[" + join_long(x) + "],y:[" + gjoin(pb) +
+         "],name: '% accumulated bases',type:'bar',line:{color:'rgba(128,128,0,1.0)', width:1}\n};\n";
+    s += "var data = [readNum, baseNum];;\n";
+    s += "var layout={legend: {x: 0, y: 1.0},title:'Read median quality distribution', xaxis:{title:'read median quality score'}, "
+         "yaxis:{title:'Percent (%)'}};\n";
+    s += "Plotly.newPlot('plot_median_qual_hist_" + div + "', data, layout);\n";
+    s += "</script>\n";
+}
+
+std::string kmer_td(const HtmlBlock& b, int i, int j, const char* letters) {   // Stats::makeKmerTD
+    const long val = b.tail[FPL_STATS_KMER + (i << 4) + j];
+    const char kmer[6] = {letters[(i >> 4) & 3], letters[(i >> 2) & 3], letters[i & 3], letters[(j >> 2) & 3], letters[j & 3], 0};
+    const double meanBases = (double)(b.bases + 1) / 2048;     // mKmerBufLen = 2 << (5 * 2): twice the 5-mers
+    const double prop = val / meanBases;
+    int r = 0, g = 0, bl = 0;
+    if (prop <= 0.3) {
+        const double frac = prop * 2.0;
+        bl = 255 - 256 * frac;
+        g = 255 * frac;
+        r = bl * frac;
+    } else if (prop > 3.0) {
+        const double frac = 2.0 / prop;
+        r = 255 - 128 * frac;
+        g = 128 * frac;
+        bl = r * frac;
+    } else {
+        r = g = bl = 196;
+    }
+    char col[32];
+    snprintf(col, sizeof(col), "%s%x%s%x%s%x", r < 16 ? "0" : "", r, g < 16 ? "0" : "", g, bl < 16 ? "0" : "", bl);
+    return std::string("<td style='background:#") + col + "' title='" + kmer + ": " + std::to_string(val) + "\n" + gfmt(prop) +
+           " times as mean value'>" + kmer + "</td>";
+}
+
+void kmer_table(std::string& s, const std::string& type, const HtmlBlock& b, bool is_rna) {   // Stats::reportHtmlKMER
+    const std::string sub = type + ": KMER counting", div = replace_all(replace_all(sub, " ", "_"), ":", "_");
+    const char letters[4] = {'A', is_rna ? 'U' : 'T', 'C', 'G'};
+    s += "<div class='subsection_title'>" + sub + "</div>\n";
+    s += "<div  id='" + div + "'>\n";
+    s += "<div class='sub_section_tips'>Darker background means larger counts. The count will be shown on mouse over.</div>\n";
+    s += "<table class='kmer_table' style='width:680px;'>\n";
+    s += "<tr><td></td>";
+    for (int h = 0; h < 16; h++) s += std::string("<td style='color:#333333'>") + letters[(h >> 2) & 3] + letters[h & 3] + "</td>";
+    s += "</tr>\n";
+    for (int i = 0; i < 64; i++) {
+        s += std::string("<tr><td style='color:#333333'>") + letters[(i >> 4) & 3] + letters[(i >> 2) & 3] + letters[i & 3] + "</td>";
+        for (int j = 0; j < 16; j++) s += kmer_td(b, i, j, letters);
+        s += "</tr>\n";
+    }
+    s += "</table>\n</div>\n";
+}
+
+std::string section_open(const char* id, const char* title) {
+    return std::string("<div class='section_div'>\n<div class='section_title' onclick=showOrHide('") + id + "')><a name='summary'>" + title +
+           "</a></div>\n<table id='" + id + "' class='section_table'>\n<tr><td>\n";
+}
+
+const char* const kSectionMid = "</td><td>\n";
+const char* const kSectionClose = "</td></tr>\n</table>\n</div>\n";
+
+// The HTML_SEGS + 1 frame pieces: piece j in front of segment j, the last behind them all
+std::vector<std::string> html_frame(const fpl_options& o, const long long* cnt, const HtmlBlock b[2], const fpl_report_html_info& info) {
+    std::vector<std::string> p(1);
+    auto hole = [&] { p.emplace_back(); };
+    const std::string time_text = info.time_text, version = info.version;
+    const bool rna = info.is_rna != 0;
+    const char* type[2] = {"Before filtering", "After filtering"};
+    std::string* s = &p.back();
+    // printHeader: printJS, printCSS
+    *s += "<html><head><meta http-equiv=\"content-type\" content=\"text/html;charset=utf-8\" />";
+    *s += "<title>fastplong report at " + time_text + " </title>";
+    *s += "<script src='https://opengene.org/plotly-1.2.0.min.js'></script>\n";
+    *s += "\n<script type='text/javascript'>\n";
+    *s += "    window.Plotly || document.write('<script src=\"https://cdn.plot.ly/plotly-1.2.0.min.js\"><\\/script>')\n";
+    *s += "</script>\n";
+    *s += "\n<script type=\"text/javascript\">\n";
+    *s += "    function showOrHide(divname) {\n";
+    *s += "        div = document.getElementById(divname);\n";
+    *s += "        if(div.style.display == 'none')\n";
+    *s += "            div.style.display = 'block';\n";
+    *s += "        else\n";
+    *s += "            div.style.display = 'none';\n";
+    *s += "    }\n";
+    *s += "</script>\n";
+    static const char* const css[] = {
+        "<style type=\"text/css\">",
+        "td {border:1px solid #dddddd;padding:5px;font-size:12px;}",
+        "table {border:1px solid #999999;padding:2x;border-collapse:collapse;width:100%}",
+        ".col1 {width:240px; font-weight:bold;}",
+        ".adapter_col {width:500px; font-size:10px;}",
+        "img {padding:30px;}",
+        "#menu {font-family:Consolas, 'Liberation Mono', Menlo, Courier, monospace;}",
+        "#menu a {color:#0366d6; font-size:18px;font-weight:600;line-height:28px;text-decoration:none;font-family:-apple-system, "
+        "BlinkMacSystemFont, 'Segoe UI', Helvetica, Arial, sans-serif, 'Apple Color Emoji', 'Segoe UI Emoji', 'Segoe UI Symbol'}",
+        "a:visited {color: #999999}",
+        ".alignleft {text-align:left;}",
+        ".alignright {text-align:right;}",
+        ".figure {width:680px;height:600px;}",
+        ".header {color:#ffffff;padding:1px;height:20px;background:#000000;}",
+        ".section_title {color:#ffffff;font-size:20px;padding:5px;text-align:left;background:#663355; margin-top:10px;}",
+        ".section_table {width:100%;}",
+        ".subsection_title {font-size:16px;padding:5px;margin-top:10px;text-align:left;color:#663355}",
+        "#container {text-align:center;padding:3px 3px 3px 10px;font-family:Arail,'Liberation Mono', Menlo, Courier, monospace;}",
+        ".menu_item {text-align:left;padding-top:5px;font-size:18px;}",
+        ".highlight {text-align:left;padding-top:30px;padding-bottom:30px;font-size:20px;line-height:35px;}",
+        "#helper {text-align:left;border:1px dotted #fafafa;color:#777777;font-size:12px;}",
+        "#footer {text-align:left;padding:15px;color:#ffffff;font-size:10px;background:#663355;font-family:Arail,'Liberation Mono', Menlo, "
+        "Courier, monospace;}",
+        ".kmer_table {text-align:center;font-size:8px;padding:2px;}",
+        ".kmer_table td{text-align:center;font-size:8px;padding:0px;color:#ffffff}",
+        ".sub_section_tips {color:#999999;font-size:10px;padding-left:5px;padding-bottom:3px;}",
+        "</style>"};
+    for (const char* line : css) *s += std::string(line) + "\n";
+    *s += "</head>";
+    *s += "<body><div id='container'>";
+    // printSummary, FilterResult::reportHtml (src/filterresult.cpp:227-242)
+    *s += "\n";
+    *s += "<h3 style='text-align:left;'><a href='https://github.com/OpenGene/fastplong' target='_blank' style='color:#663355;"
+          "text-decoration:none;'>" + std::string(info.title) + "</a><a href='https://github.com/OpenGene/fastplong' target='_blank' "
+          "style='font-size:-2;text-decoration:none;'>(fastplong version v" + version + ")</a></h3>\n";
+    *s += "<div class='section_div'>\n";
+    *s += "<div class='section_title' onclick=showOrHide('summary')><a name='summary'>Summary</a> </div>\n";
+    *s += "<div id='summary'>\n";
+    *s += "<div class='subsection_title'>Filtering result</div>\n";
+    *s += "<div id='filtering_result'>\n";
+    {
+        const double total = (double)b[0].reads;
+        const long long* f = cnt + FPL_CNT_FILTER;
+        auto fr = [&](const char* key, int code) {
+            *s += row(key, format_number(f[code]) + " (" + to_str(f[code] * 100.0 / total) + "%)");
+        };
+        *s += "<table class='summary_table'>\n";
+        fr("reads passed filters:", FPL_PASS_FILTER);
+        fr("reads with low quality:", FPL_FAIL_QUALITY);
+        fr("reads with too many N:", FPL_FAIL_N_BASE);
+        if (o.length_filter_enabled) {
+            fr("reads too short:", FPL_FAIL_LENGTH);
+            if (o.length_max > 0) fr("reads too long:", FPL_FAIL_TOO_LONG);
+        }
+        if (o.complexity_enabled) fr("reads with low complexity:", FPL_FAIL_COMPLEXITY);
+        *s += "</table>\n";
+    }
+    *s += "</div>\n";
+    *s += "</div>\n";
+    *s += "</div>\n";
+    *s += section_open("basic_stat", "Basic statistics");
+    basic_info(*s, type[0], b[0]);
+    *s += kSectionMid;
+    basic_info(*s, type[1], b[1]);
+    *s += kSectionClose;
+    *s += section_open("median_qual_stat", "Median qual histogram");
+    median_hist(*s, type[0], b[0]);
+    *s += kSectionMid;
+    median_hist(*s, type[1], b[1]);
+    *s += kSectionClose;
+    // Stats::reporHtmlMedianQualLengthDensity: segments 0..3
+    *s += section_open("median_qual_length_density", "Median qual length density");
+    for (int w = 0; w < 2; w++) {
+        const std::string sub = std::string(type[w]) + ": Density plot of read median quality and read length", div = replace_all(sub, " ", "_");
+        if (w) *s += kSectionMid;
+        *s += "<div class='subsection_title'>" + sub + "</div>\n";
+        *s += "<div id='mean_qual_length_density_figure'>\n";
+        *s += "<div class='figure' id='plot_median_qual_length_density_" + div + "' style='height:400px;'></div>\n";
+        *s += "</div>\n";
+        *s += "\n<script type=\"text/javascript\">\n";
+        *s += "var density={x:[";
+        hole(); s = &p.back();
+        *s += "],y:[";
+        hole(); s = &p.back();
+        *s += "],name: '% reads',type:'histogram2dcontour',line:{color:'rgba(128,0,128,1.0)', width:1}\n};\n";
+        *s += "var data = [density];\n";
+        *s += "var layout={legend: {x: 0, y: 1.0},title:' Density plot of read median quality and read length', xaxis:{title:'read median "
+              "quality score'}, yaxis:{title:'Read length', type:'log'}};\n";
+        *s += "Plotly.newPlot('plot_median_qual_length_density_" + div + "', data, layout);\n";
+        *s += "</script>\n";
+    }
+    *s += kSectionClose;
+    // Stats::reportHtmlQuality / reportHtmlContents: segments 4..25
+    const std::string t = rna ? "U" : "T";
+    const std::string qnames[5] = {"A", t, "C", "G", "mean"}, cnames[6] = {"A", t, "C", "G", "N", "GC"};
+    const char* const qcolors[5] = {"rgba(128,128,0,1.0)", "rgba(128,0,128,1.0)", "rgba(0,255,0,1.0)", "rgba(0,0,255,1.0)", "rgba(20,20,20,1.0)"};
+    const char* const ccolors[6] = {"rgba(128,128,0,1.0)", "rgba(128,0,128,1.0)", "rgba(0,255,0,1.0)", "rgba(0,0,255,1.0)",
+                                    "rgba(255, 0, 0, 1.0)", "rgba(20,20,20,1.0)"};
+    for (int content = 0; content < 2; content++) {
+        *s += content ? section_open("contents_stat", "Base contents statistics") : section_open("quality_stat", "Quality statistics");
+        for (int w = 0; w < 2; w++) {
+            const HtmlBlock& B = b[w];
+            const std::string sub = std::string(type[w]) + (content ? ": base contents" : ": quality");
+            const std::string div = replace_all(replace_all(sub, " ", "_"), ":", "_");
+            if (w) *s += kSectionMid;
+            *s += "<div class='subsection_title'>" + sub + "</div>\n";
+            *s += "<div id='" + div + "'>\n";
+            *s += "<div class='sub_section_tips'>Value of each position will be shown on mouse over.</div>\n";
+            *s += "<div class='figure' id='plot_" + div + "'></div>\n";
+            *s += "</div>\n";
+            *s += "\n<script type=\"text/javascript\">\n";
+            *s += "var data=[";
+            const std::string xs = join_long(B.x);
+            for (int k = 0; k < (content ? 6 : 5); k++) {
+                std::string name = content ? cnames[k] : qnames[k];
+                if (content) {
+                    const long count = k < 5 ? B.base_contents[cnames[k][0] & 7] : B.base_contents['G' & 7] + B.base_contents['C' & 7];
+                    std::string percentage = std::to_string((double)count * 100.0 / B.bases);
+                    if (percentage.length() > 5) percentage = percentage.substr(0, 5);
+                    name = cnames[k] + "(" + percentage + "%)";
+                }
+                *s += "{x:[" + xs + "],y:[";
+                hole(); s = &p.back();
+                *s += "],name: '" + name + "',mode:'lines',line:{color:'" + (content ? ccolors[k] : qcolors[k]) + "', width:1}\n},";
+            }
+            *s += "];\n";
+            *s += "var layout={title:'', xaxis:{title:'position'";
+            if (B.cycles > 300) *s += ",type:'log'";
+            *s += content ? "}, yaxis:{title:'base content ratios'}};\n" : "}, yaxis:{title:'quality'}};\n";
+            *s += "Plotly.newPlot('plot_" + div + "', data, layout);\n";
+            *s += "</script>\n";
+        }
+        *s += kSectionClose;
+    }
+    *s += section_open("kmer_stat", "k-mer statistics");
+    kmer_table(*s, type[0], b[0], rna);
+    *s += kSectionMid;
+    kmer_table(*s, type[1], b[1], rna);
+    *s += kSectionClose;
+    // printFooter
+    *s += "\n</div>\n";
+    *s += "<div id='footer'> ";
+    *s += "<p>" + std::string(info.command) + "</p>";
+    *s += "fastplong " + version + ", at " + time_text + " </div>";
+    *s += "</body></html>";
+    return p;
+}
+
+template <class T> int grow_t(T** p, int64_t* cap, int64_t n) { return grow_dev((void**)p, cap, (int64_t)sizeof(T) * n); }
+
+int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
+    FplHtml& h = c->html;
+    FplLists& L = c->lists;
+    h.built = false;
+    const int64_t C = c->C;
+    cudaStream_t s = c->stream;
+    // 1. total_cycles, bases and G+C (k_report_cycles), then the base-bin counts below total_cycles
+    if (!h.d_sum) CK(cudaMalloc(&h.d_sum, 22 * sizeof(unsigned long long)));
+    if (!h.d_lstat) CK(cudaMalloc(&h.d_lstat, 8 * sizeof(int)));
+    unsigned long long sum[22] = {(unsigned long long)C, 0, 0, (unsigned long long)C, 0, 0};
+    CK(cudaMemcpyAsync(h.d_sum, sum, sizeof(sum), cudaMemcpyHostToDevice, s));
+    { Timed t(c, K_HTML_CYCLES); launch_report_cycles(c->d_stats[0], c->d_stats[1], C, h.d_sum, s); }
+    std::vector<long long> tails(2 * FPL_STATS_TAIL), cnt((size_t)c->counter_words);
+    for (int w = 0; w < 2; w++)
+        CK(cudaMemcpyAsync(tails.data() + w * FPL_STATS_TAIL, c->d_stats[w] + 16 * C, sizeof(long long) * FPL_STATS_TAIL,
+                           cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(cnt.data(), c->d_counters, sizeof(long long) * c->counter_words, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(sum, h.d_sum, 6 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    const int64_t T[2] = {(int64_t)sum[0], (int64_t)sum[3]};
+    {
+        Timed t(c, K_HTML_CYCLES);
+        for (int w = 0; w < 2; w++) launch_html_bins(c->d_stats[w], C, T[w], h.d_sum + 6 + 8 * w, s);
+        c->launches += (T[0] > 0) + (T[1] > 0) - 1;  // one k_html_bins per block with cycles
+    }
+    // 2. each list grouped by median: the entries of bins 0..127 are the density pairs, bin 128 the empty reads
+    int64_t M[2] = {0, 0}, NE[2] = {0, 0};
+    for (int w = 0; w < 2; w++) {
+        const int64_t n = L.n[w], nch = (n + HTML_CHUNK - 1) / HTML_CHUNK;
+        if (!n) continue;
+        const int64_t m = HTML_BINS * nch + 1;
+        if (grow_t(&h.d_mat, &h.cap_mat, m) || grow_t(&h.d_moff, &h.cap_moff, m) || grow_t(&h.d_grp[w], &h.cap_grp[w], n)) return -1;
+        CK(cudaMemsetAsync(h.d_mat + m - 1, 0, sizeof(long long), s));
+        { Timed t(c, K_HTML_GROUP_HIST); launch_html_hist(L.d[w], n, nch, h.d_mat, s); }
+        size_t tb = 0;
+        CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, h.d_mat, h.d_moff, m, s));
+        if (grow_dev(&h.d_tmp, &h.cap_tmp, (int64_t)tb + 256)) return -1;
+        CK(cub::DeviceScan::ExclusiveSum(h.d_tmp, tb, h.d_mat, h.d_moff, m, s));
+        { Timed t(c, K_HTML_GROUP_SCATTER); launch_html_scatter(L.d[w], n, nch, h.d_moff, h.d_grp[w], s); }
+        CK(cudaMemcpyAsync(&NE[w], h.d_moff + 128 * nch, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&M[w], h.d_moff + 129 * nch, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+    }
+    // 3. Stats::calcLengthHistogram over [0, longest read]
+    const int64_t H = c->used_cycles + 1;
+    if (grow_t(&h.d_hist, &h.cap_hist, 2 * H) || grow_t(&h.d_lwork, &h.cap_lwork, 6 * H)) return -1;
+    CK(cudaMemsetAsync(h.d_hist, 0, sizeof(unsigned long long) * 2 * H, s));
+    const int init[8] = {INT_MAX, -1, INT_MAX, INT_MAX, INT_MAX, -1, INT_MAX, INT_MAX};
+    CK(cudaMemcpyAsync(h.d_lstat, init, sizeof(init), cudaMemcpyHostToDevice, s));
+    for (int w = 0; w < 2; w++) {
+        unsigned long long* hist = h.d_hist + w * H;
+        long long *ccum = h.d_lwork + 3 * w * H, *prod = ccum + H, *pcum = prod + H;
+        Timed t(c, K_HTML_LENGTHS);
+        launch_html_lenhist(L.d[w], L.n[w], hist, s);
+        launch_html_lenprod(hist, H, prod, s);
+        size_t tb = 0;
+        CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, hist, ccum, H, s));
+        if (grow_dev(&h.d_tmp, &h.cap_tmp, (int64_t)tb + 256)) return -1;
+        CK(cub::DeviceScan::ExclusiveSum(h.d_tmp, tb, hist, ccum, H, s));
+        tb = 0;
+        CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, prod, pcum, H, s));
+        if (grow_dev(&h.d_tmp, &h.cap_tmp, (int64_t)tb + 256)) return -1;
+        CK(cub::DeviceScan::ExclusiveSum(h.d_tmp, tb, prod, pcum, H, s));
+        const long long lensum = tails[w * FPL_STATS_TAIL + FPL_STATS_LENSUM];
+        launch_html_lensearch(hist, ccum, prod, pcum, H, lensum / 2, (unsigned long long)M[w] / 2, h.d_lstat + 4 * w, s);
+        c->launches += L.n[w] ? 2 : 1;               // k_html_lenhist (with entries), k_html_lenprod, k_html_lensearch
+    }
+    int lstat[8];
+    CK(cudaMemcpyAsync(lstat, h.d_lstat, sizeof(lstat), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(sum + 6, h.d_sum + 6, 16 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    HtmlBlock b[2];
+    for (int w = 0; w < 2; w++) {
+        const long long* tl = tails.data() + w * FPL_STATS_TAIL;
+        if (M[w] != tl[FPL_STATS_READS])
+            return fail("fpl_report_html: the %s read list holds %lld reads, the Stats block %lld", w ? "post-filter" : "pre-filter",
+                        (long long)M[w], tl[FPL_STATS_READS]);
+        HtmlBlock& B = b[w];
+        B.reads = tl[FPL_STATS_READS]; B.bases = (long)sum[3 * w + 1]; B.lensum = tl[FPL_STATS_LENSUM]; B.cycles = (long)T[w];
+        for (int k = 0; k < 8; k++) B.base_contents[k] = (long)sum[6 + 8 * w + k];
+        const int* ls = lstat + 4 * w;
+        B.min_len = ls[0] == INT_MAX ? 0 : ls[0];
+        B.max_len = ls[1] < 0 ? 0 : ls[1];
+        B.median_len = ls[2] == INT_MAX ? 0 : ls[2];
+        B.n50_len = ls[3] == INT_MAX ? 0 : ls[3];
+        B.tail = tl;
+        B.x = curve_x(B.cycles);
+    }
+    // 4. the per-cycle values, then the down-sampled means
+    const int64_t R[2] = {(int64_t)b[0].x.size(), (int64_t)b[1].x.size()};
+    if (grow_t(&h.d_x, &h.cap_x, R[0] + R[1] + 1) || grow_t(&h.d_vals, &h.cap_vals, 11 * (T[0] + T[1]) + 1) ||
+        grow_t(&h.d_sums, &h.cap_sums, 11 * (R[0] + R[1]) + 1))
+        return -1;
+    std::vector<long long> xs(b[0].x);
+    xs.insert(xs.end(), b[1].x.begin(), b[1].x.end());
+    if (!xs.empty()) CK(cudaMemcpyAsync(h.d_x, xs.data(), sizeof(long long) * xs.size(), cudaMemcpyHostToDevice, s));
+    for (int w = 0; w < 2; w++) {
+        double* vals = h.d_vals + (w ? 11 * T[0] : 0);
+        if (T[w]) { Timed t(c, K_HTML_VALUES); launch_html_values(c->d_stats[w], C, T[w], info.is_rna != 0, vals, s); }
+        if (R[w]) { Timed t(c, K_HTML_SUMS); launch_html_sums(vals, T[w], h.d_x + (w ? R[0] : 0), R[w], h.d_sums + (w ? 11 * R[0] : 0), s); }
+    }
+    // 5. the frame, the size of every value and their exclusive sum
+    const std::vector<std::string> frame = html_frame(c->P.opt, cnt.data(), b, info);
+    if ((int)frame.size() != HTML_SEGS + 1) return fail("fpl_report_html: internal error (%d frame pieces)", (int)frame.size());
+    HtmlText X = {};
+    int64_t items = 0;
+    for (int j = 0; j < HTML_SEGS; j++) {
+        X.start[j] = items;
+        if (j < 4) {                   // density x, y of block j / 2
+            const int w = j / 2;
+            X.kind[j] = j % 2; X.blk[j] = w;
+            items += M[w];
+        } else {                       // quality: 4..13 = curves 0..4 of block 0, then of block 1; content: 14..25 = curves 5..10
+            const int q = j - 4, content = q >= 10;
+            const int w = content ? (q - 10) / 6 : q / 5, k = content ? 5 + (q - 10) % 6 : q % 5;
+            X.kind[j] = 2; X.blk[j] = w;
+            X.base[j] = (int64_t)k * R[w];
+            items += R[w];
+        }
+    }
+    X.start[HTML_SEGS] = items;
+    for (int w = 0; w < 2; w++) {
+        X.grp[w] = h.d_grp[w]; X.nonempty[w] = NE[w];
+        X.sums[w] = h.d_sums + (w ? 11 * R[0] : 0);
+        X.x[w] = h.d_x + (w ? R[0] : 0);
+    }
+    if (grow_t(&h.d_size, &h.cap_size, items + 1) || grow_t(&h.d_off, &h.cap_off, items + 1)) return -1;
+    CK(cudaMemsetAsync(h.d_size + items, 0, sizeof(int64_t), s));
+    if (items) { Timed t(c, K_HTML_SIZES); launch_html_sizes(X, h.d_size, s); }
+    size_t tb = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, h.d_size, h.d_off, items + 1, s));
+    if (grow_dev(&h.d_tmp, &h.cap_tmp, (int64_t)tb + 256)) return -1;
+    CK(cub::DeviceScan::ExclusiveSum(h.d_tmp, tb, h.d_size, h.d_off, items + 1, s));
+    int64_t end[HTML_SEGS];            // the running sum behind segment j
+    for (int j = 0; j < HTML_SEGS; j++)
+        CK(cudaMemcpyAsync(&end[j], h.d_off + X.start[j + 1], sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    // 6. the frame pieces at their places, the values between them
+    const int np = HTML_SEGS + 1;
+    std::vector<int64_t> src(np + 1), dst(np);
+    int64_t fbytes = 0, shift = 0;
+    for (int j = 0; j < np; j++) {
+        src[j] = fbytes;
+        dst[j] = (j ? end[j - 1] : 0) + shift;
+        shift += (int64_t)frame[j].size();
+        fbytes += (int64_t)frame[j].size();
+        if (j < HTML_SEGS) X.shift[j] = shift;
+    }
+    src[np] = fbytes;
+    const int64_t total = end[HTML_SEGS - 1] + shift;
+    const size_t tables = sizeof(int64_t) * (2 * np + 1);
+    h.h_frame.resize(tables + (size_t)fbytes);
+    memcpy(h.h_frame.data(), src.data(), sizeof(int64_t) * (np + 1));
+    memcpy(h.h_frame.data() + sizeof(int64_t) * (np + 1), dst.data(), sizeof(int64_t) * np);
+    for (int j = 0; j < np; j++) memcpy(h.h_frame.data() + tables + src[j], frame[j].data(), frame[j].size());
+    if (grow_t(&h.d_frame, &h.cap_frame, (int64_t)h.h_frame.size()) || grow_t(&h.d_text, &h.cap_text, total)) return -1;
+    CK(cudaMemcpyAsync(h.d_frame, h.h_frame.data(), h.h_frame.size(), cudaMemcpyHostToDevice, s));
+    {
+        Timed t(c, K_HTML_TEXT);
+        const int64_t* d_src = reinterpret_cast<const int64_t*>(h.d_frame);
+        launch_html_text(X, h.d_off, h.d_frame + tables, d_src, d_src + np + 1, np, h.d_text, s);
+        if (items) c->launches++;      // k_report_frame + k_html_text (only with values to print)
+    }
+    CK(cudaGetLastError());
+    h.n_bytes = total;
+    h.built = true;
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int fpl_keep_read_lists(fpl_ctx* c, int enabled) {
+    g_err[0] = 0;
+    if (!c) return fail("fpl_keep_read_lists: null context");
+    c->lists.keep = enabled != 0;
+    return 0;
+}
+
+extern "C" int fpl_report_html(fpl_ctx* c, const fpl_report_html_info* info, uint8_t* out, int64_t cap, int64_t* n_bytes) {
+    g_err[0] = 0;
+    if (!c || !info || !n_bytes) return fail("fpl_report_html: null argument");
+    *n_bytes = 0;
+    if (info->struct_size != (int32_t)sizeof(fpl_report_html_info))
+        return fail("fpl_report_html: fpl_report_html_info.struct_size %d != %d (ABI mismatch)", info->struct_size,
+                    (int)sizeof(fpl_report_html_info));
+    if (!info->version || !info->command || !info->title || !info->time_text)
+        return fail("fpl_report_html: version, command, title and time_text must not be null");
+    if (!c->lists.complete)
+        return fail("fpl_report_html: read-list capture (fpl_keep_read_lists) was off for an fpl_process_* call since fpl_create "
+                    "or fpl_reset: the lists are incomplete");
+    if (c->lists.merged)
+        return fail("fpl_report_html: fpl_allreduce_stats merged the Stats over several ranks, but not the read lists");
+    CK(cudaSetDevice(c->device));
+    std::string key = std::string(info->version) + '\0' + info->command + '\0' + info->title + '\0' + info->time_text + '\0' +
+                      (info->is_rna ? "U" : "T");
+    if (!c->html.built || c->html.key != key) {
+        if (html_build(c, *info)) { c->html.built = false; return -1; }
+        c->html.key.swap(key);
+    }
+    *n_bytes = c->html.n_bytes;
+    if (!out || cap < c->html.n_bytes) return 1;     // the text stays built: call again with room
+    CK(cudaMemcpyAsync(out, c->html.d_text, (size_t)c->html.n_bytes, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
     collect_times(c);
     return 0;

@@ -1280,3 +1280,252 @@ void launch_report_text(const ReportCurves& R, const int64_t* off, const uint8_t
     const int64_t n = R.T[0] + R.T[1];
     if (n) k_report_text<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(R, off, text);
 }
+
+// ------------------------------------------------------------------------------------------------------------------
+// fpl_report_html (HtmlReporter::report, src/htmlreporter.cpp:75-253).  What grows with the input is printed here:
+//   k_html_capture   on the processing path (fpl_keep_read_lists): appends each call's (length, median) entries of both
+//                    Stats blocks — input order, then output-read order within a read — to the context's lists
+//   k_html_hist      grouping by median, stable: per-warp 130-bin histograms of contiguous chunks (medians 0..127, empty
+//   cub scan         reads, post-filter slots without an output read), the exclusive sum of the bin-major matrix,
+//   k_html_scatter   and a scatter that ranks equal bins inside a warp by ballots, 32 entries at a time in chunk order:
+//                    mQualLength's iteration order (a map<char, vector<int>>: ascending median, then statRead order)
+//   k_html_len*      Stats::calcLengthHistogram (src/stats.cpp:377-409): a length histogram, scans of the counts and of
+//                    the int * int products (wrapped to 32 bits, as the reference's imul is), and the first keys that pass
+//   k_html_bins      mBaseContents of each bin over the block's total_cycles (the content curves' names)
+//   k_html_values    the 11 per-cycle curves (report_value), then k_html_sums: one thread per (curve, range) of
+//                    Stats::list2string's down-sampling (:550-573), the range summed in order in double
+//   k_html_sizes / cub scan / k_html_text: every value's text at its place; k_report_frame drops the host-built frame
+// ------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ int html_bin(const HtmlEntry& e) { return e.len < 0 ? 129 : e.len == 0 ? 128 : (e.med & 127); }
+
+__device__ __forceinline__ int html_itoa(long long v, char* out) {
+    char d[24];
+    int n = 0, k = 0;
+    unsigned long long a = v < 0 ? 0ull - (unsigned long long)v : (unsigned long long)v;
+    do { d[k++] = (char)('0' + a % 10); a /= 10; } while (a);
+    if (v < 0) out[n++] = '-';
+    while (k) out[n++] = d[--k];
+    return n;
+}
+
+namespace {
+
+__global__ void k_html_capture(const fpl_read_result* __restrict__ res, const int32_t* __restrict__ lens, int64_t n,
+                               const fpl_segment* __restrict__ segs, int64_t n_segs, HtmlEntry* __restrict__ pre,
+                               HtmlEntry* __restrict__ post) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const fpl_read_result& r = res[i];
+        pre[i] = HtmlEntry{lens[i], r.pre_median_qual};
+        if (!segs)
+            for (int k = 0; k < 2; k++) {
+                const bool out = k < r.n_segments && r.seg_result[k] == FPL_PASS_FILTER;
+                post[2 * i + k] = out ? HtmlEntry{r.seg_len[k], r.seg_median_qual[k]} : HtmlEntry{-1, 0};
+            }
+    }
+    if (segs)
+        for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n_segs; j += stride) {
+            const fpl_segment& s = segs[j];
+            post[j] = s.result == FPL_PASS_FILTER ? HtmlEntry{s.len, s.median_qual} : HtmlEntry{-1, 0};
+        }
+}
+
+// warp w of block b owns chunk 4b + w: mat[bin * nchunks + chunk] = its entries of that bin
+__global__ void k_html_hist(const HtmlEntry* __restrict__ e, int64_t n, int64_t nchunks, long long* __restrict__ mat) {
+    __shared__ int h[4][HTML_BINS];
+    const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t chunk = (int64_t)blockIdx.x * 4 + wid;
+    if (chunk >= nchunks) return;
+    for (int b = lane; b < HTML_BINS; b += 32) h[wid][b] = 0;
+    __syncwarp();
+    const int64_t lo = chunk * HTML_CHUNK, hi = lo + HTML_CHUNK < n ? lo + HTML_CHUNK : n;
+    for (int64_t i = lo + lane; i < hi; i += 32) atomicAdd(&h[wid][html_bin(e[i])], 1);
+    __syncwarp();
+    for (int b = lane; b < HTML_BINS; b += 32) mat[(int64_t)b * nchunks + chunk] = h[wid][b];
+}
+
+// off: the exclusive sum of mat.  32 entries at a time, in order: an entry's rank among the equal bins of lower lanes comes
+// from 8 ballots (one per bit of the bin), the lowest lane of each bin then moves that bin's cursor
+__global__ void k_html_scatter(const HtmlEntry* __restrict__ e, int64_t n, int64_t nchunks, const long long* __restrict__ off,
+                               HtmlEntry* __restrict__ out) {
+    __shared__ long long cur[4][HTML_BINS];
+    const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t chunk = (int64_t)blockIdx.x * 4 + wid;
+    if (chunk >= nchunks) return;
+    for (int b = lane; b < HTML_BINS; b += 32) cur[wid][b] = off[(int64_t)b * nchunks + chunk];
+    __syncwarp();
+    const int64_t lo = chunk * HTML_CHUNK, hi = lo + HTML_CHUNK < n ? lo + HTML_CHUNK : n;
+    for (int64_t i0 = lo; i0 < hi; i0 += 32) {
+        const int64_t i = i0 + lane;
+        const bool ok = i < hi;
+        const HtmlEntry v = ok ? e[i] : HtmlEntry{0, 0};
+        const int key = ok ? html_bin(v) : 255;
+        unsigned peers = 0xffffffffu;
+        for (int bit = 0; bit < 8; bit++) {
+            const unsigned m = __ballot_sync(0xffffffffu, (key >> bit) & 1);
+            peers &= ((key >> bit) & 1) ? m : ~m;
+        }
+        const unsigned lower = peers & ((1u << lane) - 1u);
+        if (ok) out[cur[wid][key] + __popc(lower)] = v;
+        __syncwarp();
+        if (ok && lower == 0) cur[wid][key] += __popc(peers);
+        __syncwarp();
+    }
+}
+
+__global__ void k_html_lenhist(const HtmlEntry* __restrict__ e, int64_t n, unsigned long long* __restrict__ hist) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int len = e[i].len;
+        if (len >= 0) atomicAdd(&hist[len], 1ull);
+    }
+}
+
+// totalBase += iter->first * iter->second: an int * int product, wrapped to 32 bits before it is added
+__global__ void k_html_lenprod(const unsigned long long* __restrict__ cnt, int64_t H, long long* __restrict__ prod) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < H) prod[b] = (long long)(int32_t)((uint32_t)b * (uint32_t)cnt[b]);
+}
+
+// out: min, max, median, N50 length.  A key of 0 that passes sets its value to 0, which the next key overwrites: the
+// answer is the smallest POSITIVE key whose running sum passes.
+__global__ void k_html_lensearch(const unsigned long long* __restrict__ cnt, const long long* __restrict__ ccum,
+                                 const long long* __restrict__ prod, const long long* __restrict__ pcum, int64_t H,
+                                 long long half_sum, unsigned long long half_n, int* __restrict__ out) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= H || cnt[b] == 0) return;
+    atomicMin(&out[0], (int)b);
+    atomicMax(&out[1], (int)b);
+    if (b == 0) return;
+    if ((unsigned long long)(ccum[b] + (long long)cnt[b]) > half_n) atomicMin(&out[2], (int)b);
+    if (pcum[b] + prod[b] > half_sum) atomicMin(&out[3], (int)b);
+}
+
+// out[b] += the block's count of base bin b over cycles [0, T)
+__global__ void k_html_bins(const unsigned long long* __restrict__ blk, int64_t C, int64_t T, unsigned long long* __restrict__ out) {
+    unsigned long long s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < T; c += (int64_t)gridDim.x * blockDim.x)
+        for (int b = 0; b < 8; b++) s[b] += blk[b * C + c];
+    for (int b = 0; b < 8; b++) {
+        unsigned long long v = s[b];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+        if (lane_id() == 0 && v) atomicAdd(&out[b], v);
+    }
+}
+
+__global__ void k_html_values(const unsigned long long* __restrict__ blk, int64_t C, int64_t T, int is_rna, double* __restrict__ vals) {
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < 11 * T; t += (int64_t)gridDim.x * blockDim.x)
+        vals[t] = report_value(blk, C, t % T, (int)(t / T), is_rna);
+}
+
+// sums[k * R + i] = the mean of curve k over [x[i - 1], x[i]) (x[-1] = 0), the adds in the reference's order; the division is
+// the only non-add and is off the chain.  An empty range (k_html_text prints "0.0" for it) is left 0.
+__global__ void k_html_sums(const double* __restrict__ vals, int64_t T, const long long* __restrict__ x, int64_t R,
+                            double* __restrict__ sums) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= 11 * R) return;
+    const int64_t k = t / R, i = t % R;
+    const long long start = i ? x[i - 1] : 0, end = x[i];
+    const double* v = vals + k * T;
+    double total = 0.0;
+#pragma unroll 8
+    for (long long j = start; j < end; j++) total += v[j];
+    sums[t] = end == start ? 0.0 : total / (double)(end - start);
+}
+
+__device__ __forceinline__ int html_seg(const HtmlText& H, int64_t i) {
+    int s = 0;
+    while (s + 1 < HTML_SEGS && H.start[s + 1] <= i) s++;
+    return s;
+}
+
+__device__ __forceinline__ int html_value(const HtmlText& H, int s, int64_t i, char* buf) {
+    const int w = H.blk[s];
+    if (H.kind[s] == 2) {
+        const long long* x = H.x[w];
+        if (x[i] == (i ? x[i - 1] : 0)) { buf[0] = '0'; buf[1] = '.'; buf[2] = '0'; return 3; }     // list2string: end == start
+        return fmt_g6(H.sums[w][H.base[s] + i], buf);
+    }
+    long long v = 0;                                  // the reference's unset tail of the density arrays: 0 here
+    if (i < H.nonempty[w]) {
+        const HtmlEntry e = H.grp[w][i];
+        v = H.kind[s] == 0 ? (long long)(short)(e.med - 33) : (long long)e.len;
+    }
+    return html_itoa(v, buf);
+}
+
+__global__ void k_html_sizes(const HtmlText H, int64_t* __restrict__ size) {
+    const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= H.start[HTML_SEGS]) return;
+    const int s = html_seg(H, g);
+    char buf[24];
+    size[g] = html_value(H, s, g - H.start[s], buf) + (g + 1 < H.start[s + 1] ? 1 : 0);
+}
+
+__global__ void k_html_text(const HtmlText H, const int64_t* __restrict__ off, uint8_t* __restrict__ text) {
+    const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= H.start[HTML_SEGS]) return;
+    const int s = html_seg(H, g);
+    char buf[24];
+    const int n = html_value(H, s, g - H.start[s], buf);
+    uint8_t* dst = text + off[g] + H.shift[s];
+    for (int b = 0; b < n; b++) dst[b] = (uint8_t)buf[b];
+    if (g + 1 < H.start[s + 1]) dst[n] = ',';
+}
+
+unsigned grid_for(int64_t n, int64_t cap) {
+    const int64_t want = (n + 255) / 256;
+    return (unsigned)(want < 1 ? 1 : want < cap ? want : cap);
+}
+
+}  // namespace
+
+void launch_html_capture(const fpl_read_result* res, const int32_t* lens, int64_t n, const fpl_segment* segs, int64_t n_segs,
+                         HtmlEntry* pre, HtmlEntry* post, cudaStream_t stream) {
+    const int64_t m = n > n_segs ? n : n_segs;
+    if (m) k_html_capture<<<grid_for(m, FPL_NUM_SMS * 8), 256, 0, stream>>>(res, lens, n, segs, n_segs, pre, post);
+}
+
+void launch_html_hist(const HtmlEntry* e, int64_t n, int64_t nchunks, long long* mat, cudaStream_t stream) {
+    if (nchunks) k_html_hist<<<(unsigned)((nchunks + 3) / 4), 128, 0, stream>>>(e, n, nchunks, mat);
+}
+
+void launch_html_scatter(const HtmlEntry* e, int64_t n, int64_t nchunks, const long long* off, HtmlEntry* out, cudaStream_t stream) {
+    if (nchunks) k_html_scatter<<<(unsigned)((nchunks + 3) / 4), 128, 0, stream>>>(e, n, nchunks, off, out);
+}
+
+void launch_html_lenhist(const HtmlEntry* e, int64_t n, unsigned long long* hist, cudaStream_t stream) {
+    if (n) k_html_lenhist<<<grid_for(n, FPL_NUM_SMS * 8), 256, 0, stream>>>(e, n, hist);
+}
+
+void launch_html_lenprod(const unsigned long long* cnt, int64_t H, long long* prod, cudaStream_t stream) {
+    k_html_lenprod<<<(unsigned)((H + 255) / 256), 256, 0, stream>>>(cnt, H, prod);
+}
+
+void launch_html_lensearch(const unsigned long long* cnt, const long long* ccum, const long long* prod, const long long* pcum,
+                           int64_t H, long long half_sum, unsigned long long half_n, int* out, cudaStream_t stream) {
+    k_html_lensearch<<<(unsigned)((H + 255) / 256), 256, 0, stream>>>(cnt, ccum, prod, pcum, H, half_sum, half_n, out);
+}
+
+void launch_html_bins(const unsigned long long* blk, int64_t C, int64_t T, unsigned long long* out, cudaStream_t stream) {
+    if (T) k_html_bins<<<grid_for(T, FPL_NUM_SMS * 8), 256, 0, stream>>>(blk, C, T, out);
+}
+
+void launch_html_values(const unsigned long long* blk, int64_t C, int64_t T, int is_rna, double* vals, cudaStream_t stream) {
+    if (T) k_html_values<<<grid_for(11 * T, FPL_NUM_SMS * 16), 256, 0, stream>>>(blk, C, T, is_rna, vals);
+}
+
+void launch_html_sums(const double* vals, int64_t T, const long long* x, int64_t R, double* sums, cudaStream_t stream) {
+    if (R) k_html_sums<<<(unsigned)((11 * R + 127) / 128), 128, 0, stream>>>(vals, T, x, R, sums);
+}
+
+void launch_html_sizes(const HtmlText& H, int64_t* size, cudaStream_t stream) {
+    const int64_t n = H.start[HTML_SEGS];
+    if (n) k_html_sizes<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(H, size);
+}
+
+void launch_html_text(const HtmlText& H, const int64_t* off, const uint8_t* frame, const int64_t* src, const int64_t* dst, int n_pieces,
+                      uint8_t* text, cudaStream_t stream) {
+    k_report_frame<<<n_pieces, 256, 0, stream>>>(frame, src, dst, text);
+    const int64_t n = H.start[HTML_SEGS];
+    if (n) k_html_text<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(H, off, text);
+}

@@ -20,3 +20,28 @@ struct ReportCurves {
     int64_t shift[22];                  // curve j's text starts shift[j] bytes of frame behind its place in the scanned sizes
     int is_rna;
 };
+
+// fpl_keep_read_lists: one entry per read of a Stats block, in the order Stats::statRead saw them.  A post-filter slot that
+// holds no output read (a failing or missing segment) has len = -1; the report drops it.
+struct HtmlEntry {
+    int32_t len;
+    int32_t med;                        // the read's median quality char
+};
+
+#define HTML_CHUNK 2048                 // list entries per warp of the grouping by median
+#define HTML_BINS 130                   // its bins: medians 0..127, 128: empty reads, 129: no output read
+
+// fpl_report_html: the device-printed lists of the report, in text order — per Stats block the density x and y lists, then
+// the 5 quality and the 6 content curves of each block — between HTML_SEGS + 1 host-built frame pieces
+#define HTML_SEGS 26
+struct HtmlText {
+    int64_t start[HTML_SEGS + 1];       // index of each segment's first value; start[HTML_SEGS] = all values
+    int64_t shift[HTML_SEGS];           // frame bytes in front of the segment
+    int kind[HTML_SEGS];                // 0: density x (median - 33), 1: density y (length), 2: down-sampled curve value
+    int blk[HTML_SEGS];                 // Stats block
+    int64_t base[HTML_SEGS];            // kind 2: index of the segment's first value in sums[blk]
+    const HtmlEntry* grp[2];            // each block's list grouped by median
+    int64_t nonempty[2];                // entries of grp that are density pairs (reads with bases); the rest print 0
+    const double* sums[2];              // curve values
+    const long long* x[2];              // each block's x list: range i is [x[i - 1], x[i]), x[-1] = 0
+};

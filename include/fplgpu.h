@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define FPL_ABI_VERSION 7
+#define FPL_ABI_VERSION 8
 
 /* Filter result codes — identical to src/common.h:43-50 (they index FilterResult::mFilterReadStats[32]). */
 enum {
@@ -452,7 +452,50 @@ typedef struct fpl_report_info {
 
 int fpl_report_json(fpl_ctx* ctx, const fpl_report_info* info, uint8_t* out, int64_t cap, int64_t* n_bytes);
 
-/* Zero all accumulators (a fresh ThreadConfig); stream-ordered, asynchronous. */
+/*
+ * The per-read lists of the HTML report (Stats::mLengthVec and Stats::mQualLength, src/stats.cpp:265-375), kept on the device.
+ * Off by default.  While on, every fpl_process_host / fpl_process_device / fpl_process_fastq_host call appends to two lists,
+ * one per Stats block, each entry holding a length and a median quality char:
+ *   pre-filter   every input read, in input order (its length and pre_median_qual);
+ *   post-filter  every passing output read, in the order of fpl_emit_batch_device's `out` (input order, then segment or
+ *                --break piece order; its length and median).
+ * Capture is one more kernel at the end of each call, stream-ordered, with no host synchronisation except when a list
+ * outgrows its buffer (the buffers grow geometrically).  Lists grow with the input: 8 bytes per input read, plus 16 per input
+ * read (8 per output read with --mask / --break) for the post-filter list.  fpl_reset empties them.
+ */
+int fpl_keep_read_lists(fpl_ctx* ctx, int enabled);
+
+/*
+ * HtmlReporter::report(FilterResult, preStats, postStats) (src/htmlreporter.cpp:75-253): the exact bytes of fastplong's HTML
+ * report (-h) of this context's accumulators and read lists, under the Options the context was created with plus `info` —
+ * the report the reference writes with -w 1 (one worker: its lists are in input order).  On top of fpl_report_json's rules:
+ *   - basic statistics: Stats::calcLengthHistogram (src/stats.cpp:377-409) over the length list — minimum and maximum
+ *     length (0 without reads), median and N50 (the smallest positive length whose running read count exceeds
+ *     entries / 2, whose running sum of int * int products, each wrapped to 32 bits as the reference's compiled code does,
+ *     exceeds mLengthSum / 2); the percentages and formatNumber with the reference's own expressions (nan and inf included);
+ *   - "median qual length density": every read with bases as (median - 33, length), by ascending median, then in list order.
+ *     The reference prints mReads entries of arrays that only its reads with bases fill; the entries behind them are
+ *     uninitialised memory there and 0 here;
+ *   - quality and content curves: with total_cycles > 300 down-sampled like Stats::list2string (x = 1..40, then (int)pos for
+ *     pos *= 1.05 from 40, then total_cycles), each value the mean of its range summed in order in double;
+ *   - "reads too short" only with the length filter, "reads too long" only with a maximum length, "low complexity" only
+ *     with -y; no adapter section.
+ * Returns < 0 (with fpl_last_error) if capture was off for any fpl_process_* call since fpl_create / fpl_reset, or if the
+ * context ran fpl_allreduce_stats over more than one rank (the lists are not gathered).  The two-phase, invalidation and
+ * synchronous contract is fpl_report_json's.
+ */
+typedef struct fpl_report_html_info {
+    int32_t struct_size;              /* = sizeof(fpl_report_html_info) */
+    int32_t is_rna;                   /* as in fpl_report_info */
+    const char* version;              /* FASTPLONG_VER: the <h3> and the footer */
+    const char* command;              /* the footer's <p>, verbatim */
+    const char* title;                /* Options::reportTitle (-R), verbatim, in the <h3> */
+    const char* time_text;            /* getCurrentSystemTime()'s text: the <title> and the footer */
+} fpl_report_html_info;
+
+int fpl_report_html(fpl_ctx* ctx, const fpl_report_html_info* info, uint8_t* out, int64_t cap, int64_t* n_bytes);
+
+/* Zero all accumulators and empty the read lists (a fresh ThreadConfig); stream-ordered, asynchronous. */
 int fpl_reset(fpl_ctx* ctx);
 
 /*
