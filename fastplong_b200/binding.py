@@ -59,6 +59,7 @@ def load_library():
     lib.fpl_comm_size.argtypes = [C.c_void_p]
     lib.fpl_comm_agree_cycles.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     lib.fpl_allreduce_stats.argtypes = [C.c_void_p, C.c_int64]
+    lib.fpl_merge_stats.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int]
     lib.fpl_eval_adapter_kmers.argtypes = [C.c_int, C.POINTER(FplBatch), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                            C.POINTER(C.c_int64)]
     lib.fpl_eval_pick_adapter.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_char_p, C.c_int32]
@@ -82,6 +83,7 @@ EXPORTS = ["fpl_last_error", "fpl_abi_version", "fpl_create", "fpl_destroy", "fp
            "fpl_sync", "fpl_stream", "fpl_last_segments", "fpl_last_mask_regions", "fpl_fetch_results", "fpl_stats_cycles", "fpl_stats_reserve", "fpl_stats_download",
            "fpl_stats_device_ptr", "fpl_counter_words", "fpl_counters_download", "fpl_counters_device_ptr",
            "fpl_comm_unique_id", "fpl_comm_init", "fpl_comm_destroy", "fpl_comm_size", "fpl_comm_agree_cycles", "fpl_allreduce_stats",
+           "fpl_merge_stats",
            "fpl_eval_adapter_kmers", "fpl_eval_pick_adapter", "fpl_report_json", "fpl_keep_read_lists", "fpl_report_html", "fpl_reset", "fpl_last_kernel_times", "fpl_launch_count", "fpl_set_timing"]
 
 
@@ -313,6 +315,13 @@ class Engine:
         buf = np.empty(n.value, dtype=np.uint8)
         self._check(self.lib.fpl_report_html(self.h, C.byref(info), buf.ctypes.data, buf.size, C.byref(n)))
         return buf.tobytes()
+
+    def merge(self, *others):
+        """Stats::merge / FilterResult::merge of this engine and `others`, in that order, into this engine (fpl_merge_stats):
+        both Stats blocks and the counters become the sums, the read lists this engine's entries followed by each other engine's.
+        The others are not modified and may be used again at once.  Same device, options and adapters, or FplError."""
+        arr = (C.c_void_p * max(1, len(others)))(*(o.h.value if o.h else None for o in others))
+        self._check(self.lib.fpl_merge_stats(self.h, arr, len(others)))
 
     # --- multi-GPU merge (one process per GPU): Stats::merge / FilterResult::merge as NCCL all-reduces ---
     @staticmethod

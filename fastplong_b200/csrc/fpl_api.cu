@@ -81,7 +81,7 @@ static int fail(const char* fmt, ...) {
 enum { K_PRESEG, K_CYCLE_PRE, K_QUAL_PRE, K_TRIM, K_SCAN, K_FINAL, K_COUNT, K_CYCLE_POST, K_QUAL_POST, K_KMER_FIX, K_ALLREDUCE,
        K_EMIT_BATCH_SIZES, K_EMIT_BATCH_COPY, K_REPORT_CYCLES, K_REPORT_SIZES, K_REPORT_TEXT, K_QUAL_EXC, K_QHIST_FOLD,
        K_HTML_CAPTURE, K_HTML_CYCLES, K_HTML_GROUP_HIST, K_HTML_GROUP_SCATTER, K_HTML_LENGTHS, K_HTML_VALUES, K_HTML_SUMS,
-       K_HTML_SIZES, K_HTML_TEXT, K_NKERNELS };
+       K_HTML_SIZES, K_HTML_TEXT, K_MERGE_STATS, K_NKERNELS };
 // K_CYCLE_PRE: the fused pass (both Stats blocks) without --mask/--break, the pre-filter pass with it; K_CYCLE_POST: the
 // post-filter segments the fused pass did not take, or the whole --mask/--break post-filter list.  K_QUAL_EXC and
 // K_QHIST_FOLD replace K_QUAL_PRE where k_scan_jit counts the quality histograms.
@@ -93,7 +93,7 @@ static const char* const kKernelNames[K_NKERNELS] = {"k_make_preseg", "k_cycle_s
                                                      "k_read_qual(exceptions)", "k_qhist_fold",
                                                      "k_html(capture)", "k_html(cycles)", "k_html(group hist)", "k_html(group scatter)",
                                                      "k_html(lengths)", "k_html(values)", "k_html(sums)", "k_html(sizes)",
-                                                     "k_html(text)"};
+                                                     "k_html(text)", "k_merge_stats"};
 // K_HTML_CYCLES: k_report_cycles + k_html_bins; K_HTML_LENGTHS: k_html_lenhist, k_html_lenprod, k_html_lensearch
 
 // fpl_keep_read_lists: the (length, median) lists of both Stats blocks
@@ -214,8 +214,12 @@ struct fpl_ctx {
     ncclComm_t comm = nullptr;
     int comm_rank = 0, comm_size = 1;
     int64_t used_cycles = 0;            // longest read accumulated since the last fpl_reset
+    int64_t reduced_rows = 0;           // widest fpl_allreduce_stats since then: other ranks' reads may fill rows past used_cycles
     long long* d_agree = nullptr;       // device word for the all-reduce(max) of the cycle count
     long long* h_agree = nullptr;       // pinned
+    // fpl_merge_stats: the sources' table (k_merge_stats) and the event that orders the streams
+    MergeSrc* d_merge = nullptr; int64_t cap_merge = 0;
+    cudaEvent_t merge_ev = nullptr;
     struct Ev { int k; cudaEvent_t a, b; };
     std::vector<Ev> events;
     std::vector<cudaEvent_t> pool;
@@ -663,6 +667,8 @@ void fpl_destroy(fpl_ctx* c) {
     if (c->stream) cudaStreamSynchronize(c->stream);
     collect_times(c);
     for (auto e : c->pool) cudaEventDestroy(e);
+    if (c->merge_ev) cudaEventDestroy(c->merge_ev);
+    cudaFree(c->d_merge);
     cudaFree(c->d_adapters); cudaFree(c->d_alen); cudaFree(c->d_peq); cudaFree(c->d_peq16); cudaFree(c->d_acode); cudaFree(c->d_peq_long); cudaFree(c->d_pf_order);
     cudaFree(c->d_stats[0]); cudaFree(c->d_stats[1]); cudaFree(c->d_counters);
     fpl_cycle_ws_free(&c->cycle_ws);
@@ -1037,7 +1043,7 @@ int fpl_reset(fpl_ctx* c) {
     for (int w = 0; w < 2; w++)
         CK(cudaMemsetAsync(c->d_stats[w], 0, sizeof(unsigned long long) * FPL_STATS_WORDS(c->C), c->stream));
     CK(cudaMemsetAsync(c->d_counters, 0, sizeof(unsigned long long) * c->counter_words, c->stream));
-    c->used_cycles = 0;
+    c->used_cycles = 0; c->reduced_rows = 0;
     c->rep.built = false; c->html.built = false;
     c->lists.n[0] = c->lists.n[1] = 0;
     c->lists.complete = true; c->lists.merged = false;
@@ -1177,6 +1183,7 @@ int fpl_allreduce_stats(fpl_ctx* c, int64_t cycles) {
     // counts do not, so ranks need not share a capacity.  One group = one fused launch.
     c->rep.built = false; c->html.built = false;
     if (c->comm_size > 1) c->lists.merged = true;
+    if (cycles > c->reduced_rows) c->reduced_rows = cycles;
     Timed t(c, K_ALLREDUCE, false);
     CKN(nccl().GroupStart());
     for (int w = 0; w < 2; w++) {
@@ -2024,5 +2031,82 @@ extern "C" int fpl_report_html(fpl_ctx* c, const fpl_report_html_info* info, uin
     CK(cudaMemcpyAsync(out, c->html.d_text, (size_t)c->html.n_bytes, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
     collect_times(c);
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// fpl_merge_stats: Stats::merge / FilterResult::merge over [dst, src...] on one device (SingleEndProcessor::process,
+// src/seprocessor.cpp:108-121).  The accumulators are summed by k_merge_stats, the read lists appended by device copies; all of
+// it on dst's stream, between an event wait on every source's stream and a wait of every source's stream on dst's.
+// ------------------------------------------------------------------------------------------------------------------
+extern "C" int fpl_merge_stats(fpl_ctx* c, fpl_ctx* const* src, int n_src) {
+    g_err[0] = 0;
+    if (!c) return fail("fpl_merge_stats: null destination context");
+    if (n_src < 0) return fail("fpl_merge_stats: negative number of sources (%d)", n_src);
+    if (n_src > 0 && !src) return fail("fpl_merge_stats: null source list");
+    // every fpl_options field but struct_size (the first) and reserved (the last)
+    const size_t ob = offsetof(fpl_options, device), oe = offsetof(fpl_options, reserved);
+    for (int k = 0; k < n_src; k++) {
+        const fpl_ctx* s = src[k];
+        if (!s) return fail("fpl_merge_stats: source %d is null", k);
+        if (s == c) return fail("fpl_merge_stats: source %d is the destination itself", k);
+        if (s->device != c->device)
+            return fail("fpl_merge_stats: source %d is on device %d, the destination on device %d (merging across devices is not "
+                        "supported)", k, s->device, c->device);
+        if (memcmp(reinterpret_cast<const char*>(&s->P.opt) + ob, reinterpret_cast<const char*>(&c->P.opt) + ob, oe - ob))
+            return fail("fpl_merge_stats: source %d was created with other options than the destination", k);
+        if (s->adapter_str != c->adapter_str)
+            return fail("fpl_merge_stats: source %d was created with another adapter list than the destination", k);
+    }
+    if (n_src == 0) return 0;
+    CK(cudaSetDevice(c->device));
+    FplLists& L = c->lists;
+    int64_t rows = 0, used = c->used_cycles, reduced = c->reduced_rows, total[2] = {L.n[0], L.n[1]};
+    bool complete = L.complete, merged = L.merged;
+    std::vector<MergeSrc> tab((size_t)n_src);
+    for (int k = 0; k < n_src; k++) {
+        const fpl_ctx* s = src[k];
+        const int64_t r = std::max(s->used_cycles, s->reduced_rows);
+        tab[k] = MergeSrc{{s->d_stats[0], s->d_stats[1]}, s->d_counters, s->C, r};
+        rows = std::max(rows, r);
+        used = std::max(used, s->used_cycles);
+        reduced = std::max(reduced, s->reduced_rows);
+        complete = complete && s->lists.complete;
+        merged = merged || s->lists.merged;
+        for (int w = 0; w < 2; w++) total[w] += s->lists.n[w];
+    }
+    // the capacities first: they synchronise dst's stream when they grow
+    if (reserve_cycles(c, rows)) return -1;
+    if (L.keep && (grow_list(c, 0, total[0]) || grow_list(c, 1, total[1]))) return -1;
+    if (grow_t(&c->d_merge, &c->cap_merge, n_src)) return -1;
+    if (!c->merge_ev) CK(cudaEventCreateWithFlags(&c->merge_ev, cudaEventDisableTiming));
+    for (int k = 0; k < n_src; k++) {         // behind everything queued on the sources
+        CK(cudaEventRecord(c->merge_ev, src[k]->stream));
+        CK(cudaStreamWaitEvent(c->stream, c->merge_ev, 0));
+    }
+    CK(cudaMemcpyAsync(c->d_merge, tab.data(), sizeof(MergeSrc) * n_src, cudaMemcpyHostToDevice, c->stream));
+    {
+        Timed t(c, K_MERGE_STATS);
+        launch_merge_stats(c->d_stats[0], c->d_stats[1], c->d_counters, c->C, rows, c->counter_words, c->d_merge, n_src, c->stream);
+    }
+    if (L.keep) {
+        for (int w = 0; w < 2; w++) {
+            int64_t at = L.n[w];
+            for (int k = 0; k < n_src; k++) {
+                const int64_t n = src[k]->lists.n[w];
+                if (n) CK(cudaMemcpyAsync(L.d[w] + at, src[k]->lists.d[w], sizeof(HtmlEntry) * n, cudaMemcpyDeviceToDevice, c->stream));
+                at += n;
+            }
+            L.n[w] = at;
+        }
+    } else {
+        complete = false;                     // the sources' entries were not captured, as in a call with capture off
+    }
+    CK(cudaEventRecord(c->merge_ev, c->stream));
+    for (int k = 0; k < n_src; k++) CK(cudaStreamWaitEvent(src[k]->stream, c->merge_ev, 0));   // before the sources' next work
+    c->used_cycles = used; c->reduced_rows = reduced;
+    L.complete = complete; L.merged = merged;
+    c->rep.built = false; c->html.built = false;
+    CK(cudaGetLastError());
     return 0;
 }

@@ -1529,3 +1529,48 @@ void launch_html_text(const HtmlText& H, const int64_t* off, const uint8_t* fram
     const int64_t n = H.start[HTML_SEGS];
     if (n) k_html_text<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(H, off, text);
 }
+
+// ------------------------------------------------------------------------------------------------------------------
+// fpl_merge_stats (Stats::merge, src/stats.cpp:1013-1082; FilterResult::merge, src/filterresult.cpp:28-61): one thread owns
+// each destination word — rows [0, rows) of the 16 per-cycle arrays and the tail of both Stats blocks, then the counter
+// block — and adds the sources to it in list order.  No atomics; the sums do not depend on the grid.
+// ------------------------------------------------------------------------------------------------------------------
+namespace {
+
+__global__ void k_merge_stats(unsigned long long* __restrict__ pre, unsigned long long* __restrict__ post,
+                              unsigned long long* __restrict__ cnt, int64_t C, int64_t rows, int64_t cnt_words,
+                              const MergeSrc* __restrict__ src, int n_src) {
+    const int64_t per = 16 * rows + FPL_STATS_TAIL, total = 2 * per + cnt_words;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        if (i >= 2 * per) {                      // counter block
+            const int64_t k = i - 2 * per;
+            unsigned long long v = cnt[k];
+            for (int s = 0; s < n_src; s++) v += src[s].cnt[k];
+            cnt[k] = v;
+            continue;
+        }
+        const int w = i >= per;
+        const int64_t j = i - (w ? per : 0);
+        unsigned long long* d = w ? post : pre;
+        if (j >= 16 * rows) {                    // tail
+            const int64_t t = j - 16 * rows;
+            unsigned long long v = d[16 * C + t];
+            for (int s = 0; s < n_src; s++) v += src[s].blk[w][16 * src[s].C + t];
+            d[16 * C + t] = v;
+        } else {                                 // row b, cycle c: only sources whose rows reach c hold counts there
+            const int64_t b = j / rows, c = j - b * rows;
+            unsigned long long v = d[b * C + c];
+            for (int s = 0; s < n_src; s++)
+                if (c < src[s].rows) v += src[s].blk[w][b * src[s].C + c];
+            d[b * C + c] = v;
+        }
+    }
+}
+
+}  // namespace
+
+void launch_merge_stats(unsigned long long* pre, unsigned long long* post, unsigned long long* cnt, int64_t C, int64_t rows,
+                        int64_t cnt_words, const MergeSrc* src, int n_src, cudaStream_t stream) {
+    const int64_t total = 2 * (16 * rows + FPL_STATS_TAIL) + cnt_words;
+    k_merge_stats<<<grid_for(total, FPL_NUM_SMS * 8), 256, 0, stream>>>(pre, post, cnt, C, rows, cnt_words, src, n_src);
+}

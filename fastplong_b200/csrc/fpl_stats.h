@@ -2,6 +2,7 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <cuda_runtime.h>
 
 struct CycleWs {
     void* tmp = nullptr; size_t tmp_bytes = 0;
@@ -20,6 +21,18 @@ struct ReportCurves {
     int64_t shift[22];                  // curve j's text starts shift[j] bytes of frame behind its place in the scanned sizes
     int is_rna;
 };
+
+// fpl_merge_stats: one source context's accumulators, as k_merge_stats reads them
+struct MergeSrc {
+    const unsigned long long* blk[2];   // pre, post (FPL_STATS_WORDS(C) each)
+    const unsigned long long* cnt;      // counter block (the destination's counter_words)
+    int64_t C;                          // the source's capacity
+    int64_t rows;                       // rows [0, rows) of its per-cycle arrays may be non-zero
+};
+// k_merge_stats: rows [0, rows) and the tail of dst's two blocks (capacity C), and its cnt_words counters, += each of the n_src
+// sources' (a device table), in table order; one launch
+void launch_merge_stats(unsigned long long* pre, unsigned long long* post, unsigned long long* cnt, int64_t C, int64_t rows,
+                        int64_t cnt_words, const MergeSrc* src, int n_src, cudaStream_t stream);
 
 // fpl_keep_read_lists: one entry per read of a Stats block, in the order Stats::statRead saw them.  A post-filter slot that
 // holds no output read (a failing or missing segment) has len = -1; the report drops it.

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define FPL_ABI_VERSION 8
+#define FPL_ABI_VERSION 9
 
 /* Filter result codes — identical to src/common.h:43-50 (they index FilterResult::mFilterReadStats[32]). */
 enum {
@@ -393,6 +393,29 @@ int fpl_comm_agree_cycles(fpl_ctx* ctx, int64_t* cycles);
 int fpl_allreduce_stats(fpl_ctx* ctx, int64_t cycles);
 
 /*
+ * Several contexts in one process, on one device — Stats::merge (src/stats.cpp:1013-1082) and FilterResult::merge
+ * (src/filterresult.cpp:28-61) over the list [dst, src[0], ..., src[n_src - 1]], as SingleEndProcessor::process applies them to
+ * its workers' ThreadConfigs in thread order (src/seprocessor.cpp:108-121).  The result is left in dst:
+ *   accumulators  every word of both Stats blocks and of the counter block of dst becomes the sum over the list: what one context
+ *                 would hold had it processed dst's input and then each source's in turn.  dst's capacity grows like
+ *                 fpl_stats_reserve to cover every row a source can hold non-zero (its longest read, or the cycles of an
+ *                 fpl_allreduce_stats on it); dst's longest read becomes the longest over the list;
+ *   read lists    (fpl_keep_read_lists) each of dst's two lists becomes dst's entries followed by each source's, in src order
+ *                 (Stats::merge concatenates mLengthVec and mQualLength the same way).  The lists are complete only if every
+ *                 context's are; a dst with capture off copies none and is then incomplete, like after an fpl_process_* call
+ *                 with capture off; a context merged across ranks (fpl_allreduce_stats) still cannot report HTML.  dst's
+ *                 capture switch does not change;
+ *   reports       the JSON and HTML text built on dst is invalidated.
+ * The sources are not modified.  dst's last-call state (fpl_emit_*, fpl_last_segments, fpl_fetch_results) stays its own, and a
+ * later fpl_process_* on dst accumulates and appends behind the merged entries.  The call is ordered on dst's stream behind all
+ * work queued on each source's stream, and each source's stream then waits for the merge: a source may be processed further,
+ * reset or destroyed as soon as the call returns.  No host synchronisation, except when dst's Stats capacity or a read list grows.
+ * Refused (< 0, dst unchanged) for a null dst or source, n_src < 0, dst among the sources, a source on another device, or a source
+ * created with other fpl_options (any field but struct_size and reserved) or another adapter list.  n_src == 0 does nothing.
+ */
+int fpl_merge_stats(fpl_ctx* dst, fpl_ctx* const* src, int n_src);
+
+/*
  * SURVEY §8f row 4 — the counting half of Evaluator::evalAdapterAndReadNum (src/evaluator.cpp:105-265), context-free
  * because it runs before the adapters (and so the context) exist: over the reads of a HOST batch (the caller passes what
  * the reference would load: the first <= 64 Ki reads / 512 Mbases of the input) count the ten-mers of the first
@@ -438,7 +461,7 @@ int fpl_eval_pick_adapter(const uint32_t* counts, const uint64_t* position_acc, 
  *     with polyX trimming on
  * Two phases, like fpl_emit_fastq_host: *n_bytes is always set; with out == NULL or cap < *n_bytes the call returns 1 and
  * writes nothing — the text stays built on the device (for the same info), so a second call with room only copies.  Any later
- * call that changes the accumulators (fpl_process_*, fpl_reset, fpl_allreduce_stats, fpl_stats_reserve) invalidates the
+ * call that changes the accumulators (fpl_process_*, fpl_reset, fpl_allreduce_stats, fpl_merge_stats into it, fpl_stats_reserve) invalidates the
  * built text; writes through fpl_stats_device_ptr / fpl_counters_device_ptr are not seen until one of those calls.
  * Synchronous.  Returns 0, 1, or < 0 on error.  The drop-in binary keeps the reference's own JsonReporter.
  */
