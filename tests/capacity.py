@@ -23,16 +23,55 @@ S, E = synth.ADAPTER_START, synth.ADAPTER_END
 # name -> source file of its #define
 DEFINES = {"FPL_NUM_SMS": "fpl_device.cuh", "CS_TILE": "fpl_stats.cu", "CS_GROUP": "fpl_stats.cu", "CS_STAGE": "fpl_stats.cu",
            "KF_WARPS": "fpl_stats.cu", "KF_LONG": "fpl_stats.cu", "KF_LIST": "fpl_stats.cu", "RQ_WARPS": "fpl_stats.cu",
-           "RQ_LONG": "fpl_stats.cu", "RQ_LIST": "fpl_stats.cu"}
-# kernel -> (source file, text in front of its grid-cap expression): grid = min(want, FPL_NUM_SMS * factor)
+           "RQ_LONG": "fpl_stats.cu", "RQ_LIST": "fpl_stats.cu", "HTML_CHUNK": "fpl_stats.h"}
+# kernel -> (source file, text in front of its grid-cap expression): grid = min(want, FPL_NUM_SMS * factor), written out or as
+# grid_for(n, FPL_NUM_SMS * factor)
 GRID_CAPS = {"k_kmer_fix": ("fpl_stats.cu", "void launch_kmer_fix("), "k_read_qual": ("fpl_stats.cu", "void launch_read_qual("),
              "k_read_qual_exc": ("fpl_stats.cu", "void launch_read_qual_exc("),
-             "k_fastq_pack": ("fpl_ingest.cu", "k_fastq_pack<<<"), "k_emit_copy": ("fpl_emit.cu", "k_emit_copy<<<")}
+             "k_fastq_pack": ("fpl_ingest.cu", "k_fastq_pack<<<"), "k_emit_copy": ("fpl_emit.cu", "k_emit_copy<<<"),
+             "k_emit_batch_copy": ("fpl_emit.cu", "k_emit_batch_copy<<<"),
+             "k_report_cycles": ("fpl_stats.cu", "void launch_report_cycles("),
+             "k_html_capture": ("fpl_stats.cu", "void launch_html_capture("),
+             "k_html_lenhist": ("fpl_stats.cu", "void launch_html_lenhist("),
+             "k_html_bins": ("fpl_stats.cu", "void launch_html_bins("),
+             "k_html_values": ("fpl_stats.cu", "void launch_html_values("),
+             "k_merge_stats": ("fpl_stats.cu", "void launch_merge_stats(")}
+CAP_RE = re.compile(r"want < FPL_NUM_SMS \* (\d+) \? want : FPL_NUM_SMS \* (\d+)"
+                    r"|grid_for\([^()]*(?:\([^()]*\))?[^()]*, FPL_NUM_SMS \* (\d+)\)")
 
 
 def _sources(texts=None):
     files = set(DEFINES.values()) | {f for f, _ in GRID_CAPS.values()}
     return {f: (texts or {}).get(f) or open(os.path.join(CSRC, f)).read() for f in files}
+
+
+def _split_top(s):
+    """the comma-separated arguments of s at bracket depth 0"""
+    out, depth, cur = [], 0, ""
+    for ch in s:
+        depth += (ch in "([{") - (ch in ")]}")
+        if ch == "," and depth == 0:
+            out.append(cur.strip())
+            cur = ""
+        else:
+            cur += ch
+    return out + [cur.strip()]
+
+
+def _cap_spans(src):
+    """kernel -> (file, anchor, launch, end) of GRID_CAPS: where its anchor and its `kernel<<<` start, where the launch
+    configuration ends"""
+    out = {}
+    for kern, (fn, anchor) in GRID_CAPS.items():
+        text = src[fn]
+        i = text.find(anchor)
+        if i < 0:
+            raise AssertionError(f"{anchor} not found in {fn}")
+        k = text.find(kern + "<<<", i)
+        if k < 0:
+            raise AssertionError(f"no launch of {kern} behind {anchor} in {fn}")
+        out[kern] = (fn, i, k, text.index(">>>", k))
+    return out
 
 
 def _define_re(name):
@@ -55,21 +94,31 @@ def constants(texts=None):
         if len(m) != 1:
             raise AssertionError(f"#define {name} not found exactly once in {fn}")
         out[name] = _value(m[0][1])
-    for kern, (fn, anchor) in GRID_CAPS.items():
+    for kern, (fn, i, k, j) in _cap_spans(src).items():
         text = src[fn]
-        i = text.find(anchor)
-        if i < 0:
-            raise AssertionError(f"{anchor} not found in {fn}")
-        j = text.index(">>>", text.index(kern + "<<<", i))
-        m = re.search(r"want < FPL_NUM_SMS \* (\d+) \? want : FPL_NUM_SMS \* (\d+)", text[i:j])
-        if not m or m.group(1) != m.group(2):
-            raise AssertionError(f"the grid cap of {kern} (min(want, FPL_NUM_SMS * k)) not found in {fn}")
-        out[kern + "_BLOCKS"] = out["FPL_NUM_SMS"] * int(m.group(1))
-        launch = text[text.index(kern + "<<<", i):j + 3]
-        threads = launch.split(",")[1].strip()
+        caps = list(CAP_RE.finditer(text[i:j]))
+        if len(caps) != 1 or (caps[0].group(1) and caps[0].group(1) != caps[0].group(2)):
+            raise AssertionError(f"the grid cap of {kern} (min(want, FPL_NUM_SMS * k) or grid_for(n, FPL_NUM_SMS * k)) not found "
+                                 f"exactly once in {fn}")
+        out[kern + "_BLOCKS"] = out["FPL_NUM_SMS"] * int(caps[0].group(1) or caps[0].group(3))
+        threads = _split_top(text[k + len(kern) + 3:j])[1]
         threads = threads.replace("KF_WARPS", str(out["KF_WARPS"])).replace("RQ_WARPS", str(out["RQ_WARPS"]))
         out[kern + "_WARPS"] = _value(threads) // 32
     assert out["k_kmer_fix_WARPS"] == out["KF_WARPS"] and out["k_read_qual_WARPS"] == out["k_read_qual_exc_WARPS"] == out["RQ_WARPS"]
+    return out
+
+
+def uncapped(texts=None):
+    """(file, line) of every `FPL_NUM_SMS *` in fastplong_b200/csrc/*.cu outside the spans GRID_CAPS reads: a grid cap no
+    capacity test knows of.  texts: {file name: source text} replacing files."""
+    names = sorted(f for f in os.listdir(CSRC) if f.endswith(".cu"))
+    src = {f: (texts or {}).get(f) or open(os.path.join(CSRC, f)).read() for f in set(names) | set(_sources(texts))}
+    spans = _cap_spans(src).values()
+    out = []
+    for fn in names:
+        for m in re.finditer(r"FPL_NUM_SMS\s*\*", src[fn]):
+            if not any(f == fn and i <= m.start() < j for f, i, _, j in spans):
+                out.append((fn, src[fn].count("\n", 0, m.start()) + 1))
     return out
 
 
@@ -527,3 +576,195 @@ def check_text(eng, opt, batch, what):
     for w in (0, 1):
         compare_stats(eng.stats(w, cyc), o.stats(w, cyc), f"{what}/stats{w}")
     compare_stats(eng.counters(), o.counters(), what + "/counters")
+
+
+# ---- the report and merge kernels (fpl_report_json, fpl_report_html, fpl_merge_stats) ----
+# every read passes whole: the post-filter list is the pre-filter one with a slot of no output read (bin 129) behind each read
+REPORT_OPT = Options(disable_adapter_trimming=True, disable_quality_filtering=True, length_required=0)
+# trimmed ends: the post-filter Stats have fewer cycles than the pre-filter ones
+CURVE_OPT = Options(disable_adapter_trimming=True, disable_quality_filtering=True, length_required=1, trim_front=3, trim_tail=5)
+# every read fails: a post-filter block without cycles
+FAIL_OPT = Options(disable_adapter_trimming=True, disable_quality_filtering=True, length_required=1000)
+
+
+def html_bins(entries):
+    """k_html_hist's bin of each (length, median) entry: the median, 128 an empty read, 129 a slot without an output read"""
+    return [129 if L < 0 else 128 if L == 0 else m & 127 for L, m in entries]
+
+
+def post_slots(res):
+    """the post-filter entries k_html_capture writes without --mask/--break: two slots per record"""
+    out = []
+    for r in res:
+        for k in range(2):
+            ok = k < int(r["n_segments"]) and r["seg_result"][k] == abi.PASS_FILTER
+            out.append((int(r["seg_len"][k]), int(r["seg_median_qual"][k])) if ok else (-1, 0))
+    return out
+
+
+def warp_rounds(bins, chunk):
+    """the 32-entry rounds of k_html_scatter: chunks of `chunk` entries, each cut into rounds from its start"""
+    return [bins[lo:min(lo + 32, c + chunk, len(bins))] for c in range(0, len(bins), chunk)
+            for lo in range(c, min(c + chunk, len(bins)), 32)]
+
+
+def grouping_lengths(k):
+    """pre-filter list lengths around one chunk and one block of k_html_hist / k_html_scatter, and one of 5 blocks and more whose
+    chunk count is no multiple of 4"""
+    ch = k["HTML_CHUNK"]
+    return [ch - 1, ch, ch + 1, 4 * ch, 4 * ch + 1, 21 * ch + 17]
+
+
+def _binned_read(rng, b, j):
+    """occurrence j of bin b (0..128) as a read: median b (every quality byte b), a length of its own within the bin"""
+    if b == 128:
+        return b"", b""
+    L = 1 + 2 * j + (b & 1)
+    return _bases(rng, L), bytes([b]) * L
+
+
+def grouping_batch(k, n, seed):
+    """n reads whose entries fill bins 0..128 over every chunk and block (129 is the post-filter list's empty slots).  The first
+    round of every other chunk c is, by c / 2 % 3: 0 one bin on all its lanes, 1 distinct bins, 2 medians 0 and 1 beside
+    empty reads (bins 0 / 128 side by side; in the post-filter list 1 / 129).  Entries of one bin have distinct lengths, so a
+    reordering within a bin changes the density plot's y list."""
+    rng = np.random.default_rng(seed)
+    ch = k["HTML_CHUNK"]
+    bins = [(i * 53) % 129 for i in range(n)]
+    for c in range(0, (n + ch - 1) // ch, 2):
+        lo, hi, p = c * ch, min(c * ch + 32, (c + 1) * ch, n), c // 2 % 3
+        for i in range(lo, hi):
+            bins[i] = (7 * c) % 129 if p == 0 else (c + 5 * (i - lo)) % 129 if p == 1 else (0, 128, 1, 128)[(i - lo) % 4]
+    seen = {}
+    reads = []
+    for b in bins:
+        reads.append(_binned_read(rng, b, seen.get(b, 0)))
+        seen[b] = seen.get(b, 0) + 1
+    return pack_reads(reads)
+
+
+def capture_cap_batch(k, seed):
+    """more reads than k_html_capture's and k_html_lenhist's capped grids have threads (the lists past their caps), lengths
+    0..12 with every median"""
+    rng = np.random.default_rng(seed)
+    n = max(k["k_html_capture_BLOCKS"], k["k_html_lenhist_BLOCKS"]) * 256 + 3 * 32 + 5
+    return pack_reads([_binned_read(rng, int(b), int(rng.integers(0, 6))) for b in rng.integers(0, 129, size=n)])
+
+
+# name -> (the reads' lengths, options): ties of Stats::calcLengthHistogram's strict > and its edges
+LENGTH_CASES = {"median_tie": ([10, 20, 10, 20], REPORT_OPT),            # count at 10 = 2 = 4 / 2
+                "n50_tie": ([50, 100, 50], REPORT_OPT),                  # 50 * 2 = 100 = 200 / 2
+                "empty_only": ([0, 0, 0], REPORT_OPT), "single": ([37], REPORT_OPT), "one_length": ([25] * 6, REPORT_OPT),
+                "post_empty": ([30, 45, 0], FAIL_OPT)}
+
+
+def length_ties(lens):
+    """(the running count meets half the entries exactly at a key, the running sum of length * count meets half the length
+    sum exactly at a positive key)"""
+    lens = [L for L in lens if L >= 0]
+    keys, cnt, prod = sorted(set(lens)), 0, 0
+    med = n50 = False
+    for L in keys:
+        cnt += lens.count(L)
+        prod += L * lens.count(L)
+        med |= cnt == len(lens) // 2
+        n50 |= L > 0 and prod == sum(lens) // 2
+    return med, n50
+
+
+def length_batch(lens, seed):
+    rng = np.random.default_rng(seed)
+    return pack_reads([(_bases(rng, L), _quals(rng, L, 5, 40)) for L in lens])
+
+
+def curve_totals(k):
+    """longest reads (total cycles) on both sides of the 300-cycle down-sampling, none a multiple of 32, and one past the caps
+    of k_report_cycles / k_html_bins (cap * 256 cycles) and k_html_values (11 * cycles > cap * 256); last, a read exactly as long
+    as the library's first capacity (1024): the pre-filter block has no empty cycle, total_cycles == C"""
+    past = max(k["k_report_cycles_BLOCKS"], k["k_html_bins_BLOCKS"]) * 256 + 37
+    return [40, 41, 300, 301, max(past, k["k_html_values_BLOCKS"] * 256 // 11 + 37), 1024]
+
+
+def curve_batch(total, seed):
+    """reads of 1..total bases under CURVE_OPT, the longest exactly total"""
+    rng = np.random.default_rng(seed)
+    lens = [total, 1, 9] + [int(v) for v in rng.integers(1, total + 1, size=12)]
+    return pack_reads([(_bases(rng, L), _quals(rng, L, 1, 60)) for L in lens])
+
+
+def merge_sources(k, seed):
+    """three batches for three contexts of three capacities (the library's first is 1024 cycles, it doubles): a longest read of
+    exactly 1024 (rows == C), of 1500 and one past k_merge_stats' cap (2 * 16 * rows words > cap * 256 threads, and > 2048).
+    Their read counts are no multiples of HTML_CHUNK: the merged lists' source boundaries fall inside chunks."""
+    rng = np.random.default_rng(seed)
+    ch = k["HTML_CHUNK"]
+    longest = [1024, 1500, max(2100, k["k_merge_stats_BLOCKS"] * 256 // 32 + 101)]
+    counts = [ch // 2 + 3, ch + 5, ch // 3 + 7]
+    out = []
+    for L, n in zip(longest, counts):
+        lens = [L] + [int(v) for v in rng.integers(0, 200, size=n - 1)]
+        out.append(pack_reads(_shuffled(rng, [(_bases(rng, x), _quals(rng, x, 1, 60)) for x in lens])))
+    return out
+
+
+REPORT_TIME = "2026-10-16      12:00:00"
+
+
+def _same_text(got, want, what):
+    if got != want:
+        i = next((i for i in range(min(len(got), len(want))) if got[i] != want[i]), min(len(got), len(want)))
+        raise AssertionError(f"{what}: differs at byte {i} of {len(got)} / {len(want)}:\n"
+                             f"library: {got[max(0, i - 160):i + 60]!r}\ntwin:    {want[max(0, i - 160):i + 60]!r}")
+
+
+def check_reports(eng, opt, lists, what):
+    """the JSON and the HTML report of eng against the twins (tests/report_twin.py, tests/report_html_twin.py) over eng's own
+    accumulators and the oracle's lists (pre, post)"""
+    import report_html_twin
+    import report_twin
+    st = (eng.stats(0), eng.stats(1), eng.counters())
+    _same_text(eng.report_json(), report_twin.report(*st, opt), what + "/json")
+    _same_text(eng.report_html(time_text=REPORT_TIME), report_html_twin.report(*st, opt, *lists, time_text=REPORT_TIME), what + "/html")
+
+
+def report_run(eng, opt, batches, what):
+    """eng (fresh, lists kept) processes the batches; records, both Stats blocks and the counters against the oracle's over the
+    same batches, both reports against the twins.  Returns (the oracle's records of the last batch, the oracle's lists)."""
+    import report_html_twin
+    eng.keep_read_lists(True)
+    o = OracleEngine(opt)
+    ext = opt.mask or opt.break_reads
+    lists = ([], [])
+    for j, b in enumerate(batches):
+        res = o.process(b)
+        compare_results(eng.process(b), res, f"{what}/{j}")
+        pre, post = report_html_twin.read_lists(b.lens, res, o.segments() if ext else None)
+        if ext:
+            compare_lists(eng.segments(), o.segments(), f"{what}/{j}/segments")
+        lists[0].extend(pre)
+        lists[1].extend(post)
+    cyc = max([1] + [int(b.lens.max()) for b in batches if b.n_reads])
+    for w in (0, 1):
+        compare_stats(eng.stats(w, cyc), o.stats(w, cyc), f"{what}/stats{w}")
+    compare_stats(eng.counters(), o.counters(), what + "/counters")
+    check_reports(eng, opt, lists, what)
+    return res, lists
+
+
+# the post-filter list is fpl_ext_run's list of output reads: --mask with a start adapter (a split read gives two), --break without
+# adapters (a read of low quality only gives none)
+MASK_OPT = Options(start_adapter=S, mask=True, disable_quality_filtering=True, length_required=0)
+BREAK_OPT = Options(disable_adapter_trimming=True, break_reads=True, break_window_size=25, break_mean_quality=12,
+                    disable_quality_filtering=True, length_required=0)
+
+
+def segment_batch(k, seed, above):
+    """above (MASK_OPT): split reads among short ones, more output reads than reads.  Otherwise (BREAK_OPT): more reads, and
+    more output reads, than k_html_capture's capped grid has threads, every fifth read of low quality only (no output read)."""
+    rng = np.random.default_rng(seed)
+    if above:
+        reads = [split_read(rng, 201 + 3 * i, 205 + 5 * i) for i in range(40)] + [(_bases(rng, 20 + i), _quals(rng, 20 + i)) for i in range(20)]
+        return pack_reads(_shuffled(rng, reads))
+    n = k["k_html_capture_BLOCKS"] * 256 * 5 // 4 + 100
+    return pack_reads([(_bases(rng, 30), _q(30, 2)) if i % 5 == 4 else (_bases(rng, i % 13), _quals(rng, i % 13, 20, 60))
+                       for i in range(n)])

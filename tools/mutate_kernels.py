@@ -5,7 +5,11 @@ statistics and text kernels (tests/test_capacity_shrunk.py's cases on the mutant
 counter of k_cycle_stats at its fullest).  A surviving mutant is kernel
 behaviour the parity tests do not pin — or an equivalent mutant: the one-sided filters (a filter that says "maybe" more often
 changes no result by design), min / max ties, guards that cannot fire.
-usage: python tools/mutate_kernels.py <file.cu> <n_mutants> [seed] [workers]      (internal: --battery <lib.so> [<shrunk lib.so>])"""
+--range FROM[:TO] samples the lines from the first one containing FROM to the first one after it containing TO (or the end);
+--only reports runs only the report and merge cases (tests/test_capacity_shrunk_reports.py), which are the only ones that reach
+the report / merge code: the rest of the battery calls none of fpl_report_json, fpl_report_html, fpl_merge_stats.
+usage: python tools/mutate_kernels.py <file.cu> <n_mutants> [seed] [workers] [--range FROM[:TO]] [--only reports]
+       (internal: --battery <lib.so|-> [<shrunk lib.so>] [reports])"""
 import os
 import random
 import re
@@ -23,19 +27,53 @@ OPS = [(r"<=", "<"), (r">=", ">"), (r"(?<![<>=!-])<(?![<=])", "<="), (r"(?<![<>=
 SHRUNK = "group_of_2_stages"       # tests/test_capacity_shrunk.py: the build whose capacities the battery's small cases reach
 
 
-def battery(lib, small=None):
+def shrunk_values():
+    """the shrunk constants of the battery's small build: tests/test_capacity_shrunk.py's SHRUNK build with the grouping chunk of
+    tests/test_capacity_shrunk_reports.py"""
+    import test_capacity_shrunk as CS
+    import test_capacity_shrunk_reports as R
+    v = dict(CS.BUILDS[SHRUNK], **R.SHRUNK)
+    assert v["FPL_NUM_SMS"] == R.SHRUNK["FPL_NUM_SMS"]
+    return v
+
+
+def report_cases(small):
+    """tests/test_capacity_shrunk_reports.py's cases on the mutant's shrunk build"""
+    import capacity
+    import test_capacity_shrunk_reports as R
+    R.LIBS["lib"] = (small, capacity.constants(capacity.shrunk_sources(**shrunk_values())))
+    R.test_down_sampled_ranges_are_never_empty()
+    for which in range(len(capacity.grouping_lengths(R.LIBS["lib"][1]))):
+        R.test_grouping_by_median_across_chunks_and_blocks(which)
+    for kind in ("slots", "segments_above", "segments_below"):
+        R.test_lists_past_the_capture_cap(kind)
+    for name in sorted(capacity.LENGTH_CASES):
+        R.test_length_statistics_ties_and_edges(name)
+    for which in range(len(capacity.curve_totals(R.LIBS["lib"][1]))):
+        R.test_curves_down_sampling_and_past_the_grid_caps(which)
+    R.test_merge_three_capacities_past_the_merge_cap()
+    R.test_emit_batch_copy_more_reads_than_warps()
+
+
+def battery(lib, small=None, only=None):
     import signal
     import simt_emu
-    simt_emu._emu_lib_path = lib
+    if lib != "-":
+        simt_emu._emu_lib_path = lib
     import capacity
     import cases
     import test_capacity_shrunk as CS
     import test_simt_kernels as T
-    signal.alarm(900)
+    signal.alarm(300 if only == "reports" else 900)        # the report cases take well under a minute
     try:
+        if only == "reports":
+            report_cases(small)
+            print("SURVIVED")
+            return
         # the capacity limits: the mutant built with shrunk constants, and the packed counter at its fullest at full size
         if small:
-            CS.LIBS[SHRUNK] = (small, capacity.constants(capacity.shrunk_sources(**CS.BUILDS[SHRUNK])))
+            report_cases(small)
+            CS.LIBS[SHRUNK] = (small, capacity.constants(capacity.shrunk_sources(**shrunk_values())))
             for optset in sorted(capacity.CS_SETS):
                 CS.test_cycle_stats_staging_rounds_and_groups(SHRUNK, optset)
                 CS.test_cycle_stats_post_filter_counts(SHRUNK, optset)
@@ -67,7 +105,16 @@ def battery(lib, small=None):
         print("KILLED (%s)" % type(e).__name__)
 
 
-def candidates(text):
+def line_range(text, spec):
+    """[first, last) line indices of --range FROM[:TO]"""
+    lines = text.split("\n")
+    frm, _, to = spec.partition(":")
+    a = next(i for i, ln in enumerate(lines) if frm in ln)
+    b = next((i for i in range(a + 1, len(lines)) if to in lines[i]), len(lines)) if to else len(lines)
+    return a, b
+
+
+def candidates(text, rng_lines=None):
     out = []
     in_comment = False
     for li, line in enumerate(text.split("\n")):
@@ -84,6 +131,8 @@ def candidates(text):
         st = code.strip()
         if not st or st.startswith("#") or st.startswith("template") or "static_assert" in st or "<<<" in st or "asm" in st:
             continue
+        if rng_lines and not rng_lines[0] <= li < rng_lines[1]:
+            continue
         for pat, rep in OPS:
             for m in re.finditer(pat, code):
                 out.append((li, m.start(), m.end(), rep))
@@ -93,40 +142,48 @@ def candidates(text):
 def run_one(args):
     import capacity
     import simt_emu
-    import test_capacity_shrunk
-    k, fn, text, (li, a, b, rep) = args
+    k, fn, text, (li, a, b, rep), only = args
     lines = text.split("\n")
     new = lines[li][:a] + rep + lines[li][b:]
     mutated = "\n".join(lines[:li] + [new] + lines[li + 1:])
     try:
-        lib = simt_emu.build_library({fn: mutated})
-        small = simt_emu.build_library(capacity.shrunk_sources({fn: mutated}, **test_capacity_shrunk.BUILDS[SHRUNK]))
+        lib = simt_emu.build_library({fn: mutated}) if only != "reports" else "-"
+        small = simt_emu.build_library(capacity.shrunk_sources({fn: mutated}, **shrunk_values()))
     except Exception:
         return k, "nocompile", lines[li], new
     try:
-        p = subprocess.run([sys.executable, os.path.abspath(__file__), "--battery", lib, small], capture_output=True, text=True,
-                           timeout=1200)
+        p = subprocess.run([sys.executable, os.path.abspath(__file__), "--battery", lib, small] + ([only] if only else []),
+                           capture_output=True, text=True, timeout=1200)
         out = p.stdout.strip().split("\n")[-1] if p.stdout.strip() else "KILLED (crash)"
     except subprocess.TimeoutExpired:
         out = "KILLED (timeout)"
-    subprocess.run(["rm", "-rf", os.path.dirname(lib), os.path.dirname(small)])
+    subprocess.run(["rm", "-rf", os.path.dirname(small)] + ([os.path.dirname(lib)] if lib != "-" else []))
     return k, out, lines[li], new
 
 
 if __name__ == "__main__":
     if sys.argv[1] == "--battery":
-        battery(*sys.argv[2:4])
+        battery(*sys.argv[2:5])
         sys.exit(0)
-    fn, count = sys.argv[1], int(sys.argv[2])
-    rng = random.Random(int(sys.argv[3]) if len(sys.argv) > 3 else 1)
+    argv, flags = [], {}
+    it = iter(sys.argv[1:])
+    for a in it:
+        if a in ("--range", "--only"):
+            flags[a] = next(it)
+        else:
+            argv.append(a)
+    fn, count = argv[0], int(argv[1])
+    rng = random.Random(int(argv[2]) if len(argv) > 2 else 1)
     text = open(os.path.join(ROOT, "fastplong_b200", "csrc", fn)).read()
-    cand = candidates(text)
+    span = line_range(text, flags["--range"]) if "--range" in flags else None
+    cand = candidates(text, span)
     picks = rng.sample(cand, min(count, len(cand)))
-    print(f"{fn}: {len(cand)} candidate mutants, running {len(picks)}", flush=True)
+    print(f"{fn}: {len(cand)} candidate mutants" + (f" in lines {span[0] + 1}..{span[1]}" if span else "") + f", running {len(picks)}",
+          flush=True)
     tally = {}
-    with ThreadPoolExecutor(int(sys.argv[4]) if len(sys.argv) > 4 else 6) as ex:
-        for k, out, old, new in ex.map(run_one, [(k, fn, text, c) for k, c in enumerate(picks)]):
+    with ThreadPoolExecutor(int(argv[3]) if len(argv) > 3 else 6) as ex:
+        for k, out, old, new in ex.map(run_one, [(k, fn, text, c, flags.get("--only")) for k, c in enumerate(picks)]):
             tally[out.split(" ")[0]] = tally.get(out.split(" ")[0], 0) + 1
             if out.startswith("SURVIVED"):
-                print(f"SURVIVED  {old.strip()[:110]}   ==>   {new.strip()[:110]}", flush=True)
+                print(f"SURVIVED  line {picks[k][0] + 1}: {old.strip()[:110]}   ==>   {new.strip()[:110]}", flush=True)
     print(tally)
