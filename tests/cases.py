@@ -515,3 +515,117 @@ def random_case_long_reads(rng):
     seed = rng.randint(1, 10**6)
     batch = synth.ont_like(rng.randint(3, 8), rng.choice([60000, 150000]), seed, p_chimera=0.6, q_mean=rng.choice([12.0, 18.0, 30.0]))
     return Options(**kw), batch, f"long {kw} seed={seed}"
+
+
+# ---- --mask / --break at the edges of fpl_ext.cu: pieces on the length limits, filter ties counted on the masked copy, region
+# walks that start at base 0 / end on the last base, more output reads than the record's two inline slots ----
+# The reference's rolling sum holds w - 1 bytes (Filter::detectLowQualityRegions, SURVEY A.8): a window is low unless its bytes
+# average about (33 + Q) * w / (w - 1), and after the first region the sum restarts from 0, so a later region ends only where a
+# window of very low bytes is followed by one of high bytes.  The quality palette below is built around that.
+MASK_BREAK_EDGE_SETS = {
+    # pieces of length_required / length_limit and one either side; --mean_qual with bytes below '!'
+    "break_lengths_mean": Options(disable_adapter_trimming=True, break_reads=True, break_window_size=4, break_mean_quality=10,
+                                  length_required=6, length_limit=14, mean_qual=20, unqualified_percent_limit=100,
+                                  n_percent_limit=100),
+    # -n and the N share on the masked copy, -u with bytes exactly on -q
+    "mask_n_limits": Options(disable_adapter_trimming=True, mask=True, mask_window_size=3, mask_mean_quality=12, n_base_limit=4,
+                             n_percent_limit=30, qualified_quality_phred=20, unqualified_percent_limit=50, length_required=1),
+    # both stages, -y ties on the masked copy and on 1- / 2-base pieces, the N share
+    "mask_break_cplx": Options(disable_adapter_trimming=True, mask=True, mask_window_size=2, mask_mean_quality=20, break_reads=True,
+                               break_window_size=3, break_mean_quality=8, low_complexity_filter=True, complexity_threshold=50,
+                               length_required=0, n_percent_limit=50),
+    # -q 0 / -u 0 under --break
+    "break_q0_u0": Options(disable_adapter_trimming=True, break_reads=True, break_window_size=5, break_mean_quality=12,
+                           qualified_quality_phred=0, unqualified_percent_limit=0, length_required=1),
+    # complexity with neither the quality nor the length filter (no counts taken), one-base windows
+    "cplx_only_w1": Options(disable_adapter_trimming=True, mask=True, mask_window_size=1, mask_mean_quality=30, break_reads=True,
+                            break_window_size=6, break_mean_quality=8, disable_quality_filtering=True,
+                            disable_length_filtering=True, low_complexity_filter=True, complexity_threshold=40),
+    # the quality filter without the length filter (the counts are taken when either is on), one-base break windows (regions of
+    # one base: first == last)
+    "break_w1_qual_only": Options(disable_adapter_trimming=True, break_reads=True, break_window_size=1, break_mean_quality=20,
+                                  disable_length_filtering=True, unqualified_percent_limit=30, n_percent_limit=20),
+    # split reads (a start adapter in the middle) broken on either side
+    "split_break_mask": Options(start_adapter=S, end_adapter=E, trimming_extension=0, mask=True, mask_window_size=6,
+                                mask_mean_quality=18, break_reads=True, break_window_size=8, break_mean_quality=10,
+                                length_required=5, low_complexity_filter=True, complexity_threshold=30),
+}
+
+
+def mask_break_edge_batch(seed=11, n=700):
+    """Short reads (mostly 1..90 bases) whose qualities are blocks of high (73, 127), very low (1..5, below '!'), low-but-printable
+    (34..40) and near-threshold bytes, windows of the sets above at both ends of a read, whole reads of high bytes (no region) and
+    of low bytes (vanishing reads), sequences of two letters with runs of N (complexity and N ties, masked N next to N), long reads
+    (pieces over 32 bases), and split reads (a start adapter in the middle of 600 bases).  The read count is no multiple of 8."""
+    rng = np.random.default_rng(seed)
+    reads = []
+
+    def qblock(k, kind):
+        if kind == 0:
+            return bytes([73]) * k
+        if kind == 1:
+            return bytes([127]) * k
+        if kind == 2:
+            return bytes(rng.integers(1, 6, size=k).astype(np.uint8))
+        if kind == 3:
+            return bytes(rng.integers(34, 41, size=k).astype(np.uint8))
+        return bytes(rng.integers(40, 60, size=k).astype(np.uint8))
+
+    def qual(L):
+        q = b""
+        while len(q) < L:
+            q += qblock(int(rng.integers(1, 12)), int(rng.choice(5, p=[0.3, 0.2, 0.25, 0.15, 0.1])))
+        return q[:L]
+
+    def seq(L):
+        a, c = rng.choice(list(b"ACGT"), size=2, replace=False)
+        p = rng.choice([0.1, 0.3, 0.5, 0.7])
+        s, cur = bytearray(), int(a)
+        for _ in range(L):
+            s.append(cur)
+            if rng.random() < p:
+                cur = int(c) if cur == int(a) else int(a)
+        for _ in range(int(rng.integers(0, 3))):
+            if L:
+                at, k = int(rng.integers(0, L)), int(rng.integers(1, 4))
+                s[at:at + k] = b"N" * len(s[at:at + k])
+        return bytes(s)
+
+    for k in range(n - 64):
+        L = int(rng.integers(1, 91)) if k % 10 else int(rng.integers(1, 8))
+        reads.append((seq(L), qual(L)))
+    for L in (1, 2, 3, 5, 8, 13):
+        reads.append((seq(L), bytes([127]) * L))                   # no region
+        reads.append((seq(L), bytes([3]) * L))                     # low everywhere: vanishes
+    for L in (3, 4):                                               # at most one window (no region): sums of q - 33 on a mean of
+        for total in (20 * L, 20 * L - 1, 21 * L - 1, -L):         # 20 (the --mean_qual of the sets), below it, negative
+            q = [33 + total // L] * L
+            q[0] += total - L * (total // L)
+            reads.append((seq(L), bytes(q)))
+    for q in (b"4\x7f5\x7f54\x7f5\x7f55\x7f", b"\x7f\x7f54\x7f55\x7f5", b"\x7f55\x7f4\x7f55\x7f4"):   # -q 20 ('5'): the
+        reads.append((seq(len(q)), q))                             # bytes on it decide -u 50 (no mask region at w 3, Q 12)
+    for q in ((2, 60, 118), (3, 3, 60, 118), (2, 60, 2, 60, 118)):  # one-base windows: a rise of 58 ends a region at once
+        reads.append((seq(len(q)), bytes(q)))
+    for L, k in ((10, 3), (10, 4), (20, 6), (20, 5)):              # the N share on 30 % and above it, on unmasked bases
+        sq = bytearray(seq(L).replace(b"N", b"A"))
+        sq[1:2 * k:2] = b"N" * k
+        reads.append((bytes(sq), bytes([127]) * L))
+    for k in range(16):                                            # pieces over 32 bases: the warp loops
+        L = int(rng.integers(100, 400))
+        q = bytearray(bytes([127]) * L)
+        for at in rng.integers(0, L, size=3):
+            q[int(at):int(at) + 12] = bytes([2]) * len(q[int(at):int(at) + 12])
+        reads.append((seq(L), bytes(q)))
+    for k in range(18):                                            # split reads, broken on the left, the right or both; a
+        la, lb = 240 + 7 * k, 300 + 5 * k                          # region that ends near a side's end leaves a tail piece
+        qa, qb = bytearray(bytes([73]) * la), bytearray(bytes([73]) * lb)
+        t = 2 + k % 7
+        if k % 3 != 1:
+            qa[la - 30 - t:la - t] = bytes([2]) * 30
+            qa[la - t:] = bytes([127]) * t
+        if k % 3 != 0:
+            qb[lb - 20 - t:lb - t] = bytes([2]) * 20
+            qb[lb - t:] = bytes([127]) * t
+        reads.append((seq(la) + S.encode() + seq(lb), bytes(qa) + bytes([73]) * len(S) + bytes(qb)))
+    assert len(reads) % 8 and len(reads) % 256
+    return pack_reads(reads)

@@ -1,8 +1,9 @@
 """TEST INFRASTRUCTURE: the kernels' own arithmetic helpers, compiled for the HOST from the source text of the .cu files.
 
 The bit-parallel edit distances (Myers32 / myers16 / myers64 / myers128 / myers_long), the search-mode lower-bound filter
-(SearchMyers), the exact byte classifiers (is_acgt, encode4's ACGTU test, kmer_code) and passFilter's integer forms
-(pass_filter) are plain integer C++ inside `__device__` functions.  This module cuts their definitions out of
+(SearchMyers), the exact byte classifiers (is_acgt, encode4's ACGTU test, kmer_code), passFilter's integer forms (pass_filter,
+and fpl_ext.cu's own copy pass_filter_ext) and the --mask / --break region walk (detect_regions, walk_break, the clamp of the mask
+kernels) are plain integer C++ inside `__device__` functions.  This module cuts their definitions out of
 fastplong_b200/csrc/*.cu / *.cuh by name, rewrites the two inline-PTX forms they use (`mad.lo.u32`) as C, and builds them
 with g++ behind small shims (`__device__` -> nothing, `__ldg`, `__dp4a`, `uint4`) into /tmp — so that the CPU tests run the
 very text the GPU runs, over input spaces the GPU tests can only sample (every byte value, ties of every threshold,
@@ -294,6 +295,98 @@ def load_qual_step():
     lib = C.CDLL(so)
     for f in (lib.j_qual_words, lib.f_qual_words):
         f.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    return lib
+
+
+# ---- the --mask / --break stage (fpl_ext.cu): its own passFilter copy, the region detection, the break walk and the clamp of
+# maskRegionWithN, in a translation unit of their own (fpl_scan.cu has a `struct Counts` too) ----
+EXT_WANTED = [("sq", "func"), ("detect_regions", "func"), ("walk_break", "func"), ("Counts", "struct"), ("pass_filter_ext", "func")]
+
+EXT_HARNESS = r"""
+extern "C" {
+int e_pass_filter(const fpl_options* o, int rlen, int lowq, int nn, int totalq, int diff) {
+    Counts c = {lowq, nn, totalq, diff};
+    return pass_filter_ext(*o, rlen, c);
+}
+// n quality strings of l bytes each (stride l), window w, quality Q.  Per string i, with at most maxr regions / pieces:
+//   nreg[i], reg[i][k] = (first, last)            detect_regions as it emits them
+//   npc[i], pc[i][k] = (lo, len, break index)      walk_break (-1: no region, the read stays whole)
+//   nmask[i], mreg[i][k] = (start, len)            k_ext_mask_count's count and k_ext_mask_emit's clamped regions
+//   mseq[i][0..l)                                  'A' everywhere, 'N' where k_ext_mask_emit paints
+void e_regions(const uint8_t* qs, int n, int l, int w, int Q, int maxr, int* nreg, int* reg, int* npc, int* pc, int* nmask,
+               int* mreg, uint8_t* mseq) {
+    for (int i = 0; i < n; i++) {
+        const uint8_t* q = qs + (size_t)i * l;
+        int k = 0;
+        nreg[i] = detect_regions(q, l, w, Q, [&](int first, int last) {
+            if (k < maxr) { reg[((size_t)i * maxr + k) * 2] = first; reg[((size_t)i * maxr + k) * 2 + 1] = last; }
+            k++;
+        });
+        k = 0;
+        npc[i] = walk_break(q, l, w, Q, [&](int plo, int plen, int bidx) {
+            if (k < maxr) { int* p = pc + ((size_t)i * maxr + k) * 3; p[0] = plo; p[1] = plen; p[2] = bidx; }
+            k++;
+        });
+        {   // k_ext_mask_count
+            const int length = l;
+            int n = 0;
+            detect_regions(q, length, w, Q, [&](int first, int last) {
+@@MASK_COUNT@@
+            });
+            nmask[i] = n;
+        }
+        {   // k_ext_mask_emit
+            const int length = l;
+            uint8_t* base = mseq + (size_t)i * l;
+            memset(base, 'A', l);
+            struct { int read, lo; } sg = {0, 0};
+            fpl_region regs[64], *out = regs;
+            detect_regions(q, length, w, Q, [&](int first, int last) {
+@@MASK_EMIT@@
+            });
+            for (int k2 = 0; k2 < (int)(out - regs) && k2 < maxr; k2++) {
+                mreg[((size_t)i * maxr + k2) * 2] = regs[k2].lo; mreg[((size_t)i * maxr + k2) * 2 + 1] = regs[k2].len;
+            }
+        }
+    }
+}
+}
+"""
+
+
+def _mask_lambda(kernel_text, what):
+    """the body of the region lambda a mask kernel hands to detect_regions"""
+    return _one(r"detect_regions\(b\.qual[^\n]*\[&\]\(int first, int last\) \{\n(.*?)\n\s*\}\);", kernel_text, what)
+
+
+def ext_source():
+    path = os.path.join(CSRC, "fpl_ext.cu")
+    parts = [SHIMS]
+    for name, kind in EXT_WANTED:
+        parts.append(f"// ---- {name} (fpl_ext.cu) ----\n" + extract(path, name, kind))
+    count = _mask_lambda(extract(path, "k_ext_mask_count", "func"), "the region lambda of k_ext_mask_count")
+    emit = _mask_lambda(extract(path, "k_ext_mask_emit", "func"), "the region lambda of k_ext_mask_emit")
+    parts.append(EXT_HARNESS.replace("@@MASK_COUNT@@", count).replace("@@MASK_EMIT@@", emit))
+    return "\n".join(parts)
+
+
+_ext_lib = None
+
+
+def load_ext():
+    global _ext_lib
+    if _ext_lib is not None:
+        return _ext_lib
+    src = ext_source()
+    so = f"/tmp/fpl_ext_helpers_{hashlib.md5(src.encode()).hexdigest()[:12]}.so"
+    if not os.path.exists(so):
+        cpp = so[:-3] + ".cpp"
+        open(cpp, "w").write(src)
+        subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", "-I", os.path.join(ROOT, "include"), "-o", so, cpp])
+    lib = C.CDLL(so)
+    lib.e_pass_filter.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.e_regions.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 7
+    _ext_lib = lib
     return lib
 
 

@@ -152,7 +152,7 @@ def _reference_pass_filter(o, rlen, lowq, nn, totalq, diff):
     if o.qual_filter_enabled:
         if lowq > (o.unqualified_percent_limit * rlen / 100.0):
             return abi.FAIL_QUALITY
-        if o.avg_qual_req > 0 and (totalq // rlen) < o.avg_qual_req:
+        if o.avg_qual_req > 0 and (abs(totalq) // rlen * (1 if totalq >= 0 else -1)) < o.avg_qual_req:   # C int division
             return abi.FAIL_QUALITY
         if nn * 100 > rlen * o.n_base_percent_limit:
             return abi.FAIL_N_BASE
@@ -171,17 +171,13 @@ def _reference_pass_filter(o, rlen, lowq, nn, totalq, diff):
     return abi.PASS_FILTER
 
 
-def test_pass_filter_integer_forms_on_every_tie(lib):
-    """k_final's pass_filter (integer products) against the reference's double forms: for every read length up to 400 and
-    every percentage 0..100, the count sitting exactly on each threshold and its two neighbours; then random counts and
-    lengths up to 2 000 000."""
+def pass_filter_tie_space():
+    """(fpl_options, rlen, lowq, nn, totalq, diff): for every read length up to 400 and every percentage 0..100, the count
+    sitting exactly on each threshold and its two neighbours; the mean-quality ties; then random counts and lengths up to
+    2 000 000."""
     def abi_opts(**kw):
         o, ad, keep = Options(disable_adapter_trimming=True, **kw).to_abi()
         return o
-
-    def same(o, rlen, lowq, nn, totalq, diff):
-        got = lib.h_pass_filter(C.byref(o), rlen, lowq, nn, totalq, diff)
-        assert got == _reference_pass_filter(o, rlen, lowq, nn, totalq, diff), (rlen, lowq, nn, totalq, diff)
 
     lens = list(range(1, 401))
     for pct in range(0, 101):
@@ -192,18 +188,17 @@ def test_pass_filter_integer_forms_on_every_tie(lib):
             edge = pct * (rlen - 1) // 100
             for d in (edge - 1, edge, edge + 1):
                 if 0 <= d <= rlen - 1:
-                    same(oc, rlen, 0, 0, 40 * rlen, d)
+                    yield oc, rlen, 0, 0, 40 * rlen, d
             edge = pct * rlen // 100
             for k in (edge - 1, edge, edge + 1):
                 if 0 <= k <= rlen:
-                    same(ou, rlen, k, 0, 40 * rlen, 0)
-                    same(on, rlen, 0, k, 40 * rlen, 0)
-    for req in (1, 7, 20, 40):
+                    yield ou, rlen, k, 0, 40 * rlen, 0
+                    yield on, rlen, 0, k, 40 * rlen, 0
+    for req in (0, 1, 7, 20, 40):       # a negative totalQual (bytes below '!') too: no --mean_qual check at 0
         o = abi_opts(mean_qual=req, length_required=0)
         for rlen in lens:
-            for t in (req * rlen - 1, req * rlen, req * rlen + 1, (req + 1) * rlen - 1):
-                if t >= 0:
-                    same(o, rlen, 0, 0, t, 0)
+            for t in (req * rlen - 1, req * rlen, req * rlen + 1, (req + 1) * rlen - 1, -1, -rlen, -rlen - 1):
+                yield o, rlen, 0, 0, t, 0
     rng = np.random.default_rng(9)
     for case in range(30000):
         o = abi_opts(low_complexity_filter=bool(rng.integers(2)), complexity_threshold=int(rng.integers(0, 101)),
@@ -213,7 +208,14 @@ def test_pass_filter_integer_forms_on_every_tie(lib):
                      disable_quality_filtering=bool(rng.integers(4) == 0), disable_length_filtering=bool(rng.integers(4) == 0)) if case % 50 == 0 else o
         rlen = int(rng.choice([rng.integers(0, 50), rng.integers(0, 5000), rng.integers(0, 2_000_000)]))
         lowq, nn = int(rng.integers(0, rlen + 1)), int(rng.integers(0, rlen // 4 + 1))
-        same(o, rlen, lowq, nn, int(rng.integers(0, 60)) * rlen + int(rng.integers(0, rlen + 1)), int(rng.integers(0, max(1, rlen))))
+        yield o, rlen, lowq, nn, int(rng.integers(0, 60)) * rlen + int(rng.integers(0, rlen + 1)), int(rng.integers(0, max(1, rlen)))
+
+
+def test_pass_filter_integer_forms_on_every_tie(lib):
+    """k_final's pass_filter (integer products) against the reference's double forms over pass_filter_tie_space()."""
+    for o, rlen, lowq, nn, totalq, diff in pass_filter_tie_space():
+        got = lib.h_pass_filter(C.byref(o), rlen, lowq, nn, totalq, diff)
+        assert got == _reference_pass_filter(o, rlen, lowq, nn, totalq, diff), (rlen, lowq, nn, totalq, diff)
 
 
 # ---- helpers of the whole-read scan k_scan_jit v2 (cut out of the raw string NVRTC compiles) ----

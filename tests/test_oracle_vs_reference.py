@@ -141,3 +141,19 @@ def test_random_option_sets(seed):
         for w in (0, 1):
             compare_stats(o.stats(w, cyc), r.stats(w, cyc), f"{what}/stats{w}")
         compare_stats(o.counters(), r.counters(), what + "/counters")
+
+
+@pytest.mark.parametrize("name", sorted(cases.MASK_BREAK_EDGE_SETS))
+def test_mask_break_edges(name):
+    """cases.MASK_BREAK_EDGE_SETS on cases.mask_break_edge_batch: pieces on the length limits, filter ties on the masked copy,
+    region walks at base 0 and the last base, split reads broken on either side, more than two output reads per read."""
+    opt, batch = cases.MASK_BREAK_EDGE_SETS[name], cases.mask_break_edge_batch()
+    o, r = OracleEngine(opt), RefEngine(opt)
+    what = f"{name}/edges"
+    compare_results(o.process(batch), r.process(batch), what)
+    compare_lists(o.segments(), r.segments(), what + "/segments")
+    compare_lists(o.mask_regions(), r.mask_regions(), what + "/regions")
+    cyc = max(1, int(batch.lens.max()))
+    for w in (0, 1):
+        compare_stats(o.stats(w, cyc), r.stats(w, cyc), f"{what}/stats{w}")
+    compare_stats(o.counters(), r.counters(), what + "/counters")

@@ -8,8 +8,10 @@ changes no result by design), min / max ties, guards that cannot fire.
 --range FROM[:TO] samples the lines from the first one containing FROM to the first one after it containing TO (or the end);
 --only reports runs only the report and merge cases (tests/test_capacity_shrunk_reports.py), which are the only ones that reach
 the report / merge code: the rest of the battery calls none of fpl_report_json, fpl_report_html, fpl_merge_stats.
-usage: python tools/mutate_kernels.py <file.cu> <n_mutants> [seed] [workers] [--range FROM[:TO]] [--only reports]
-       (internal: --battery <lib.so|-> [<shrunk lib.so>] [reports])"""
+--only ext runs only the --mask / --break cases, the only ones that reach fpl_ext.cu (fpl_ext_run runs only with one of the two
+flags on): the same verdict as the whole battery for a mutant of that file, in a fraction of the time.
+usage: python tools/mutate_kernels.py <file.cu> <n_mutants> [seed] [workers] [--range FROM[:TO]] [--only reports|ext]
+       (internal: --battery <lib.so|-> [<shrunk lib.so>] [reports|ext])"""
 import os
 import random
 import re
@@ -55,6 +57,21 @@ def report_cases(small):
     R.test_emit_batch_copy_more_reads_than_warps()
 
 
+def ext_cases(T):
+    """every case of the battery that turns --mask or --break on"""
+    import cases
+    for name, opt in cases.MASK_BREAK_SETS.items():
+        T.check(opt, cases.blocky_quality_batch(5, n=40), name)
+    edges = cases.mask_break_edge_batch()
+    for name, opt in cases.MASK_BREAK_EDGE_SETS.items():
+        T.check(opt, edges, name + "/edges")
+    T.check_text(cases.MASK_BREAK_SETS["mask_and_break"], cases.blocky_quality_batch(5, n=30), "text/ext")
+    T.check_text(cases.MASK_BREAK_EDGE_SETS["split_break_mask"], edges, "text/ext/edges")
+    for name, (opt, b) in cases.edge_cases().items():
+        if opt.mask or opt.break_reads:
+            T.check(opt, b, name)
+
+
 def battery(lib, small=None, only=None):
     import signal
     import simt_emu
@@ -64,10 +81,14 @@ def battery(lib, small=None, only=None):
     import cases
     import test_capacity_shrunk as CS
     import test_simt_kernels as T
-    signal.alarm(300 if only == "reports" else 900)        # the report cases take well under a minute
+    signal.alarm(300 if only in ("reports", "ext") else 900)       # the report cases take well under a minute
     try:
         if only == "reports":
             report_cases(small)
+            print("SURVIVED")
+            return
+        if only == "ext":
+            ext_cases(T)
             print("SURVIVED")
             return
         # the capacity limits: the mutant built with shrunk constants, and the packed counter at its fullest at full size
@@ -89,15 +110,13 @@ def battery(lib, small=None, only=None):
             T.check(cases.OPTION_SETS[name], adv, name)
         for name, opt in cases.RNA_SETS.items():
             T.check(opt, cases.rna_batch(41, n=40, mean=1000, mixed=True), name)
-        for name, opt in cases.MASK_BREAK_SETS.items():
-            T.check(opt, cases.blocky_quality_batch(5, n=40), name)
+        ext_cases(T)
         for n in (33, 65, 129):
             T.check(cases.OPTION_SETS[f"long_adapter_{n}"], cases.long_adapter_batch(n, 900 + n, n=16), f"long{n}")
         T.check(cases.OPTION_SETS["fasta64_polyx"], cases.hifi_fasta64_batch(3, n=40), "fasta64")
         from fastplong_b200 import synth
         T.check(cases.OPTION_SETS["cut_polyx_cplx"], synth.ont_like(2, 110000, 5, p_chimera=1.0), "reads beyond 96 kb")      # block-wide paths
         T.check_text(cases.OPTION_SETS["cut_polyx_cplx"], cases.adversarial_batch(3), "text")
-        T.check_text(cases.MASK_BREAK_SETS["mask_and_break"], cases.blocky_quality_batch(5, n=30), "text/ext")
         print("SURVIVED")
     except AssertionError:
         print("KILLED")
@@ -148,16 +167,16 @@ def run_one(args):
     mutated = "\n".join(lines[:li] + [new] + lines[li + 1:])
     try:
         lib = simt_emu.build_library({fn: mutated}) if only != "reports" else "-"
-        small = simt_emu.build_library(capacity.shrunk_sources({fn: mutated}, **shrunk_values()))
+        small = simt_emu.build_library(capacity.shrunk_sources({fn: mutated}, **shrunk_values())) if only != "ext" else None
     except Exception:
         return k, "nocompile", lines[li], new
     try:
-        p = subprocess.run([sys.executable, os.path.abspath(__file__), "--battery", lib, small] + ([only] if only else []),
+        p = subprocess.run([sys.executable, os.path.abspath(__file__), "--battery", lib, small or "-"] + ([only] if only else []),
                            capture_output=True, text=True, timeout=1200)
         out = p.stdout.strip().split("\n")[-1] if p.stdout.strip() else "KILLED (crash)"
     except subprocess.TimeoutExpired:
         out = "KILLED (timeout)"
-    subprocess.run(["rm", "-rf", os.path.dirname(small)] + ([os.path.dirname(lib)] if lib != "-" else []))
+    subprocess.run(["rm", "-rf"] + [os.path.dirname(p) for p in (small, lib) if p and p != "-"])
     return k, out, lines[li], new
 
 
