@@ -22,6 +22,7 @@
 #include "fpl_ingest.h"
 #include "fpl_ext.h"
 #include "fpl_emit.h"
+#include "fpl_buf.h"
 
 static_assert(sizeof(fpl_options) == 144, "fpl_options ABI size");
 static_assert(sizeof(fpl_segment) == 20 && sizeof(fpl_region) == 12, "segment / region ABI size");
@@ -98,8 +99,8 @@ static const char* const kKernelNames[K_NKERNELS] = {"k_make_preseg", "k_cycle_s
 
 // fpl_keep_read_lists: the (length, median) lists of both Stats blocks
 struct FplLists {
-    HtmlEntry* d[2] = {nullptr, nullptr};
-    int64_t cap[2] = {0, 0}, n[2] = {0, 0};
+    DevBuf<HtmlEntry> d[2];
+    int64_t n[2] = {0, 0};
     bool keep = false;                  // capture on
     bool complete = true;               // every fpl_process_* call since fpl_create / fpl_reset captured
     bool merged = false;                // fpl_allreduce_stats over more than one rank since then
@@ -107,21 +108,21 @@ struct FplLists {
 
 // fpl_report_html: the text and its work buffers
 struct FplHtml {
-    HtmlEntry* d_grp[2] = {nullptr, nullptr}; int64_t cap_grp[2] = {0, 0};
-    long long* d_mat = nullptr; int64_t cap_mat = 0;     // grouping histograms, then their exclusive sum in place
-    long long* d_moff = nullptr; int64_t cap_moff = 0;
-    unsigned long long* d_hist = nullptr; int64_t cap_hist = 0;   // length histogram
-    long long* d_lwork = nullptr; int64_t cap_lwork = 0;          // count scan, products, product scan
-    int* d_lstat = nullptr;                                       // min, max, median, N50 of each block
-    unsigned long long* d_sum = nullptr;                          // k_report_cycles' 6 words, then 16 base-bin counts
-    long long* d_x = nullptr; int64_t cap_x = 0;
-    double* d_vals = nullptr; int64_t cap_vals = 0;
-    double* d_sums = nullptr; int64_t cap_sums = 0;
-    int64_t* d_size = nullptr; int64_t cap_size = 0;
-    int64_t* d_off = nullptr; int64_t cap_off = 0;
-    void* d_tmp = nullptr; int64_t cap_tmp = 0;
-    uint8_t* d_frame = nullptr; int64_t cap_frame = 0;
-    uint8_t* d_text = nullptr; int64_t cap_text = 0;
+    DevBuf<HtmlEntry> d_grp[2];
+    DevBuf<long long> d_mat;            // grouping histograms, then their exclusive sum in place
+    DevBuf<long long> d_moff;
+    DevBuf<unsigned long long> d_hist;  // length histogram
+    DevBuf<long long> d_lwork;          // count scan, products, product scan
+    DevBuf<int> d_lstat;                // min, max, median, N50 of each block
+    DevBuf<unsigned long long> d_sum;   // k_report_cycles' 6 words, then 16 base-bin counts
+    DevBuf<long long> d_x;
+    DevBuf<double> d_vals;
+    DevBuf<double> d_sums;
+    DevBuf<int64_t> d_size;
+    DevBuf<int64_t> d_off;
+    DevBuf<uint8_t> d_tmp;
+    DevBuf<uint8_t> d_frame;
+    DevBuf<uint8_t> d_text;
     std::vector<uint8_t> h_frame;
     bool built = false;
     std::string key;
@@ -130,12 +131,12 @@ struct FplHtml {
 
 // fpl_report_json: the report text of the accumulators as they were when it was built, kept in HBM until a call changes them
 struct FplReport {
-    unsigned long long* d_sum = nullptr;            // k_report_cycles: total_cycles, bases, G+C of each block
-    int64_t* d_size = nullptr; int64_t cap_size = 0;   // bytes of every value
-    int64_t* d_off = nullptr; int64_t cap_off = 0;     // their exclusive sum
-    void* d_tmp = nullptr; int64_t cap_tmp = 0;
-    uint8_t* d_frame = nullptr; int64_t cap_frame = 0;   // piece tables + the host-built frame
-    uint8_t* d_text = nullptr; int64_t cap_text = 0;
+    DevBuf<unsigned long long> d_sum;   // k_report_cycles: total_cycles, bases, G+C of each block
+    DevBuf<int64_t> d_size;             // bytes of every value
+    DevBuf<int64_t> d_off;              // their exclusive sum
+    DevBuf<uint8_t> d_tmp;
+    DevBuf<uint8_t> d_frame;            // piece tables + the host-built frame
+    DevBuf<uint8_t> d_text;
     std::vector<uint8_t> h_frame;
     bool built = false;
     std::string key;                                // version, command and is_rna of the built text
@@ -163,46 +164,44 @@ struct fpl_ctx {
     FplReport rep;
     FplLists lists;
     FplHtml html;
-    uint8_t* d_adapters = nullptr;
-    int* d_alen = nullptr;
-    uint4* d_peq = nullptr;
-    uint32_t* d_peq16 = nullptr;
-    uint32_t* d_acode = nullptr;
-    unsigned long long* d_peq_long = nullptr;
-    int* d_pf_order = nullptr;
+    DevBuf<uint8_t> d_adapters;
+    DevBuf<int> d_alen;
+    DevBuf<uint4> d_peq;
+    DevBuf<uint32_t> d_peq16;
+    DevBuf<uint32_t> d_acode;
+    DevBuf<unsigned long long> d_peq_long;
+    DevBuf<int> d_pf_order;
     // accumulators
     int64_t C = 0;
-    unsigned long long* d_stats[2] = {nullptr, nullptr};
-    unsigned long long* d_counters = nullptr;
+    DevBuf<unsigned long long> d_stats[2];
+    DevBuf<unsigned long long> d_counters;
     int64_t counter_words = 0;
     // per-read work buffers
     int64_t cap_reads = 0;
-    ReadState* d_state = nullptr;
-    fpl_read_result* d_results = nullptr;
+    DevBuf<ReadState> d_state;
+    DevBuf<fpl_read_result> d_results;
     CycleWs cycle_ws;
-    StatSeg* d_preseg = nullptr;
-    StatSeg* d_postseg = nullptr;
+    DevBuf<StatSeg> d_preseg;
+    DevBuf<StatSeg> d_postseg;
     // k_scan_jit with the quality histograms (jit.qhist): their striped sums, and k_final's list of the reads whose one
     // passing segment is not their window (k_read_qual_exc)
-    unsigned long long* d_qstripes = nullptr;
-    int32_t* d_exc = nullptr;
-    int* d_nexc = nullptr;
+    DevBuf<unsigned long long> d_qstripes;
+    DevBuf<int32_t> d_exc;
+    DevBuf<int> d_nexc;
     int64_t last_n = 0;
     fpl_read_result* last_results = nullptr;  // where the last call's records live (device)
     // staging for host batches
-    int64_t cap_bytes = 0;
-    uint8_t* d_seq = nullptr;
-    uint8_t* d_qual = nullptr;
-    int64_t cap_idx = 0;
-    int64_t* d_offsets = nullptr;
-    int32_t* d_lens = nullptr;
+    DevBuf<uint8_t> d_seq;
+    DevBuf<uint8_t> d_qual;
+    DevBuf<int64_t> d_offsets;
+    DevBuf<int32_t> d_lens;
     std::vector<int32_t> h_lens;
     // tiling + measurement
     int64_t tile_bases = 0;
     // fpl_process_host: the upload runs on its own stream, piece by piece, and the kernels of a piece start as soon
     // as its bytes have arrived (copy/compute overlap inside one call)
     cudaStream_t copy_stream = nullptr;
-    int* d_minmax = nullptr;            // fpl_process_device: min / max read length of the batch
+    DevBuf<int> d_minmax;               // fpl_process_device: min / max read length of the batch
     int* h_minmax = nullptr;
     std::vector<cudaEvent_t> piece_events;
     int64_t piece_bytes = 16ll << 20;
@@ -215,10 +214,10 @@ struct fpl_ctx {
     int comm_rank = 0, comm_size = 1;
     int64_t used_cycles = 0;            // longest read accumulated since the last fpl_reset
     int64_t reduced_rows = 0;           // widest fpl_allreduce_stats since then: other ranks' reads may fill rows past used_cycles
-    long long* d_agree = nullptr;       // device word for the all-reduce(max) of the cycle count
+    DevBuf<long long> d_agree;          // device word for the all-reduce(max) of the cycle count
     long long* h_agree = nullptr;       // pinned
     // fpl_merge_stats: the sources' table (k_merge_stats) and the event that orders the streams
-    MergeSrc* d_merge = nullptr; int64_t cap_merge = 0;
+    DevBuf<MergeSrc> d_merge;
     cudaEvent_t merge_ev = nullptr;
     struct Ev { int k; cudaEvent_t a, b; };
     std::vector<Ev> events;
@@ -229,55 +228,56 @@ static int ensure_reads(fpl_ctx* c, int64_t n) {
     if (n <= c->cap_reads) return 0;
     int64_t cap = c->cap_reads ? c->cap_reads : 1024;
     while (cap < n) cap *= 2;
-    cudaFree(c->d_state); cudaFree(c->d_results); cudaFree(c->d_preseg); cudaFree(c->d_postseg); cudaFree(c->d_exc);
-    c->d_state = nullptr; c->d_results = nullptr; c->d_preseg = nullptr; c->d_postseg = nullptr; c->d_exc = nullptr; c->cap_reads = 0;
-    CK(cudaMalloc(&c->d_state, sizeof(ReadState) * cap));
-    CK(cudaMalloc(&c->d_results, sizeof(fpl_read_result) * cap));
-    CK(cudaMalloc(&c->d_preseg, sizeof(StatSeg) * cap));
-    CK(cudaMalloc(&c->d_postseg, sizeof(StatSeg) * 2 * cap));
-    if (c->jit.qhist) CK(cudaMalloc(&c->d_exc, sizeof(int32_t) * cap));
+    c->cap_reads = 0;
+    c->d_state.reset(); c->d_results.reset(); c->d_preseg.reset(); c->d_postseg.reset(); c->d_exc.reset();
+    CK(c->d_state.grow_exact(cap));
+    CK(c->d_results.grow_exact(cap));
+    CK(c->d_preseg.grow_exact(cap));
+    CK(c->d_postseg.grow_exact(2 * cap));
+    if (c->jit.qhist) CK(c->d_exc.grow_exact(cap));
     c->cap_reads = cap;
     return 0;
 }
 
+// Both blocks re-laid out at capacity nc, or (on any failure) the context as it was: the new blocks are allocated and filled
+// before they replace the old ones.
 static int reserve_cycles(fpl_ctx* c, int64_t need) {
     if (need <= c->C) return 0;
     c->rep.built = false; c->html.built = false;
     int64_t nc = c->C ? c->C : 1024;
     while (nc < need) nc *= 2;
+    DevBuf<unsigned long long> nb[2];
+    for (int w = 0; w < 2; w++) CK(nb[w].grow_exact(FPL_STATS_WORDS(nc)));
     for (int w = 0; w < 2; w++) {
-        unsigned long long* nb = nullptr;
-        CK(cudaMalloc(&nb, sizeof(unsigned long long) * FPL_STATS_WORDS(nc)));
-        CK(cudaMemsetAsync(nb, 0, sizeof(unsigned long long) * FPL_STATS_WORDS(nc), c->stream));
-        if (c->d_stats[w]) {
+        CK(cudaMemsetAsync(nb[w], 0, sizeof(unsigned long long) * FPL_STATS_WORDS(nc), c->stream));
+        if (c->C) {
             // rows b*C + c move to b*nc + c; the tail moves to 16*nc
-            CK(cudaMemcpy2DAsync(nb, sizeof(unsigned long long) * nc, c->d_stats[w], sizeof(unsigned long long) * c->C,
+            CK(cudaMemcpy2DAsync(nb[w], sizeof(unsigned long long) * nc, c->d_stats[w], sizeof(unsigned long long) * c->C,
                                  sizeof(unsigned long long) * c->C, 16, cudaMemcpyDeviceToDevice, c->stream));
-            CK(cudaMemcpyAsync(nb + 16 * nc, c->d_stats[w] + 16 * c->C, sizeof(unsigned long long) * FPL_STATS_TAIL,
+            CK(cudaMemcpyAsync(nb[w] + 16 * nc, c->d_stats[w] + 16 * c->C, sizeof(unsigned long long) * FPL_STATS_TAIL,
                                cudaMemcpyDeviceToDevice, c->stream));
-            CK(cudaStreamSynchronize(c->stream));
-            cudaFree(c->d_stats[w]);
         }
-        c->d_stats[w] = nb;
     }
+    if (c->C) CK(cudaStreamSynchronize(c->stream));
+    for (int w = 0; w < 2; w++) c->d_stats[w].swap(nb[w]);      // nb frees the old blocks
     c->C = nc;
     return 0;
 }
 
-// list w holds at least `need` entries, its entries kept.  Geometric, so the wait for the copy (cudaFree) is rare.
+// list w holds at least `need` entries, its entries kept
 static int grow_list(fpl_ctx* c, int w, int64_t need) {
     FplLists& L = c->lists;
-    if (need <= L.cap[w]) return 0;
-    int64_t cap = L.cap[w] ? L.cap[w] : (1 << 16);
-    while (cap < need) cap *= 2;
-    HtmlEntry* p = nullptr;
-    CK(cudaMalloc(&p, sizeof(HtmlEntry) * cap));
-    if (L.n[w]) CK(cudaMemcpyAsync(p, L.d[w], sizeof(HtmlEntry) * L.n[w], cudaMemcpyDeviceToDevice, c->stream));
-    if (L.d[w]) {
-        CK(cudaStreamSynchronize(c->stream));
-        cudaFree(L.d[w]);
-    }
-    L.d[w] = p; L.cap[w] = cap;
+    CK(L.d[w].grow_keep(need, L.n[w], c->stream, (int64_t)sizeof(HtmlEntry) << 16));
+    return 0;
+}
+
+// the staging batch of host input: n_bytes in each of seq and qual, n_reads offsets and lengths, each at exactly that size when
+// it grows
+static int reserve_staging(fpl_ctx* c, int64_t n_bytes, int64_t n_reads) {
+    CK(c->d_seq.grow_exact(n_bytes));
+    CK(c->d_qual.grow_exact(n_bytes));
+    CK(c->d_offsets.grow_exact(n_reads));
+    CK(c->d_lens.grow_exact(n_reads));
     return 0;
 }
 
@@ -415,7 +415,7 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
         if (!ext) {
             if (qhist) { Timed t(c, K_QUAL_EXC); launch_read_qual_exc(b, st, exc, c->d_nexc, c->d_stats[0], c->d_stats[1], c->C, res, s); }
             { Timed t(c, K_COUNT);
-              launch_count(res, b.n_reads, c->d_counters, true, b.lens, qhist ? c->d_stats[0] : nullptr, c->d_stats[1], c->C, s); }
+              launch_count(res, b.n_reads, c->d_counters, true, b.lens, qhist ? c->d_stats[0].get() : nullptr, c->d_stats[1], c->C, s); }
             // one pass over the reads counts the pre-filter Stats and, for the read's slot-0 passing segment, the
             // post-filter per-cycle counters; the residual pass counts the passing segments it did not take
             { Timed t(c, K_CYCLE_PRE);
@@ -456,7 +456,7 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
         if (grow_list(c, 0, L.n[0] + n) || grow_list(c, 1, L.n[1] + n_post)) return -1;
         if (n || n_post) {
             Timed t(c, K_HTML_CAPTURE);
-            launch_html_capture(d_res, full.lens, n, ext ? c->ext.d_segs : nullptr, ext ? n_post : 0, L.d[0] + L.n[0], L.d[1] + L.n[1],
+            launch_html_capture(d_res, full.lens, n, ext ? c->ext.d_segs.get() : nullptr, ext ? n_post : 0, L.d[0] + L.n[0], L.d[1] + L.n[1],
                                 c->stream);
         }
         L.n[0] += n; L.n[1] += n_post;
@@ -501,7 +501,7 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
         return fail("fpl_create: no usable CUDA device (%s); libfplgpu has no CPU fallback", cudaGetErrorString(e));
     if (opt->device < 0 || opt->device >= ndev) return fail("fpl_create: device %d out of range (%d devices)", opt->device, ndev);
     CK(cudaSetDevice(opt->device));
-    CK(cudaFree(0));
+    CK(cudaDeviceSynchronize());        // the first call that needs the device context creates it
     stamp("driver + device context");
     fpl_ctx* c = new fpl_ctx();
     c->device = opt->device;
@@ -591,18 +591,18 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
     for (int i = 0; i <= FPL_MAX_ADAPTER_LEN; i++) c->P.thr[i] = (short)(int)round(opt->ed_max * i);  // src/adaptertrimmer.cpp:73
 #define CKC(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { fail("%s failed: %s", #call, cudaGetErrorString(e_)); fpl_destroy(c); return -1; } } while (0)
     CKC(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    CKC(cudaMalloc(&c->d_adapters, h_ad.size()));
-    CKC(cudaMalloc(&c->d_alen, sizeof(int) * n));
-    CKC(cudaMalloc(&c->d_peq, sizeof(uint4) * h_peq.size()));
-    CKC(cudaMalloc(&c->d_peq16, sizeof(uint32_t) * h_peq16.size()));
-    CKC(cudaMalloc(&c->d_acode, sizeof(uint32_t) * h_acode.size()));
+    CKC(c->d_adapters.grow_exact((int64_t)h_ad.size()));
+    CKC(c->d_alen.grow_exact(n));
+    CKC(c->d_peq.grow_exact((int64_t)h_peq.size()));
+    CKC(c->d_peq16.grow_exact((int64_t)h_peq16.size()));
+    CKC(c->d_acode.grow_exact((int64_t)h_acode.size()));
     CKC(cudaMemcpy(c->d_acode, h_acode.data(), sizeof(uint32_t) * h_acode.size(), cudaMemcpyHostToDevice));
     CKC(cudaMemcpy(c->d_adapters, h_ad.data(), h_ad.size(), cudaMemcpyHostToDevice));
     CKC(cudaMemcpy(c->d_alen, h_alen.data(), sizeof(int) * n, cudaMemcpyHostToDevice));
     CKC(cudaMemcpy(c->d_peq, h_peq.data(), sizeof(uint4) * h_peq.size(), cudaMemcpyHostToDevice));
     CKC(cudaMemcpy(c->d_peq16, h_peq16.data(), sizeof(uint32_t) * h_peq16.size(), cudaMemcpyHostToDevice));
     if (peq_words) {
-        CKC(cudaMalloc(&c->d_peq_long, sizeof(unsigned long long) * h_peq_long.size()));
+        CKC(c->d_peq_long.grow_exact((int64_t)h_peq_long.size()));
         CKC(cudaMemcpy(c->d_peq_long, h_peq_long.data(), sizeof(unsigned long long) * h_peq_long.size(), cudaMemcpyHostToDevice));
     }
     c->P.peq_long = c->d_peq_long; c->P.peq_words = peq_words;
@@ -615,13 +615,13 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
                 const int kc = h_alen[k] <= 32 ? 0 : h_alen[k] <= 64 ? 1 : 2;
                 if (kc == cls) order.push_back(k);
             }
-        CKC(cudaMalloc(&c->d_pf_order, sizeof(int) * order.size()));
+        CKC(c->d_pf_order.grow_exact((int64_t)order.size()));
         CKC(cudaMemcpy(c->d_pf_order, order.data(), sizeof(int) * order.size(), cudaMemcpyHostToDevice));
     }
     c->P.pf_order = c->d_pf_order;
     c->P.adapters = c->d_adapters; c->P.alen = c->d_alen; c->P.peq = c->d_peq; c->P.peq16 = c->d_peq16; c->P.acode = c->d_acode;
     c->counter_words = FPL_COUNTER_WORDS(n);
-    CKC(cudaMalloc(&c->d_counters, sizeof(unsigned long long) * c->counter_words));
+    CKC(c->d_counters.grow_exact(c->counter_words));
     CKC(cudaMemset(c->d_counters, 0, sizeof(unsigned long long) * c->counter_words));
     stamp("tables");
     // specialise the scan kernel on the adapters (NVRTC); FPL_NO_JIT=1 keeps the precompiled k_scan_fast
@@ -640,8 +640,8 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
         }
     }
     if (c->jit.qhist) {
-        CKC(cudaMalloc(&c->d_qstripes, sizeof(unsigned long long) * QH_STRIPES * 256));
-        CKC(cudaMalloc(&c->d_nexc, sizeof(int)));
+        CKC(c->d_qstripes.grow_exact(QH_STRIPES * 256));
+        CKC(c->d_nexc.grow_exact(1));
         c->P.qstripes = c->d_qstripes;
     }
     stamp("scan kernel specialisation");
@@ -668,33 +668,13 @@ void fpl_destroy(fpl_ctx* c) {
     collect_times(c);
     for (auto e : c->pool) cudaEventDestroy(e);
     if (c->merge_ev) cudaEventDestroy(c->merge_ev);
-    cudaFree(c->d_merge);
-    cudaFree(c->d_adapters); cudaFree(c->d_alen); cudaFree(c->d_peq); cudaFree(c->d_peq16); cudaFree(c->d_acode); cudaFree(c->d_peq_long); cudaFree(c->d_pf_order);
-    cudaFree(c->d_stats[0]); cudaFree(c->d_stats[1]); cudaFree(c->d_counters);
-    fpl_cycle_ws_free(&c->cycle_ws);
     for (auto e : c->piece_events) cudaEventDestroy(e);
-    cudaFree(c->d_minmax); if (c->h_minmax) cudaFreeHost(c->h_minmax);
+    if (c->h_minmax) cudaFreeHost(c->h_minmax);
     fpl_comm_destroy(c);
-    cudaFree(c->d_agree); if (c->h_agree) cudaFreeHost(c->h_agree);
+    if (c->h_agree) cudaFreeHost(c->h_agree);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-    cudaFree(c->d_state); cudaFree(c->d_results); cudaFree(c->d_preseg); cudaFree(c->d_postseg);
-    cudaFree(c->d_qstripes); cudaFree(c->d_exc); cudaFree(c->d_nexc);
-    cudaFree(c->d_seq); cudaFree(c->d_qual); cudaFree(c->d_offsets); cudaFree(c->d_lens);
-    fpl_ingest_free(&c->ingest);
-    fpl_ext_free(&c->ext);
-    fpl_emit_free(&c->emit);
-    fpl_emit_batch_free(&c->bemit);
-    cudaFree(c->rep.d_sum); cudaFree(c->rep.d_size); cudaFree(c->rep.d_off); cudaFree(c->rep.d_tmp); cudaFree(c->rep.d_frame);
-    cudaFree(c->rep.d_text);
-    {
-        FplHtml& h = c->html;
-        for (int w = 0; w < 2; w++) { cudaFree(c->lists.d[w]); cudaFree(h.d_grp[w]); }
-        cudaFree(h.d_mat); cudaFree(h.d_moff); cudaFree(h.d_hist); cudaFree(h.d_lwork); cudaFree(h.d_lstat); cudaFree(h.d_sum);
-        cudaFree(h.d_x); cudaFree(h.d_vals); cudaFree(h.d_sums); cudaFree(h.d_size); cudaFree(h.d_off); cudaFree(h.d_tmp);
-        cudaFree(h.d_frame); cudaFree(h.d_text);
-    }
     if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
+    delete c;                           // the device buffers go with their owners
 }
 
 int fpl_process_device(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results_dev) {
@@ -709,10 +689,8 @@ int fpl_process_device(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results_
     // to know: reduce them on the side stream, which does not wait for the kernels of the previous batch still running
     // on the compute stream
     if (!c->copy_stream) CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-    if (!c->d_minmax) {
-        CK(cudaMalloc(&c->d_minmax, 4 * sizeof(int)));
-        CK(cudaMallocHost(&c->h_minmax, 4 * sizeof(int)));
-    }
+    CK(c->d_minmax.grow_exact(4));
+    if (!c->h_minmax) CK(cudaMallocHost(&c->h_minmax, 4 * sizeof(int)));
     c->h_minmax[0] = 0; c->h_minmax[1] = 0; c->h_minmax[2] = 0;
     if (n) {
         const int init[3] = {INT_MAX, INT_MIN, 0};
@@ -767,18 +745,7 @@ int fpl_process_host(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results) {
                         (long long)i, (long long)o, b->lens[i], (long long)b->n_bytes);
     }
     const int64_t need = FPL_BATCH_BYTES(b->n_bytes);  // the tail the kernels' whole-vector reads may touch
-    if (need > c->cap_bytes) {
-        cudaFree(c->d_seq); cudaFree(c->d_qual); c->d_seq = c->d_qual = nullptr; c->cap_bytes = 0;
-        CK(cudaMalloc(&c->d_seq, need));
-        CK(cudaMalloc(&c->d_qual, need));
-        c->cap_bytes = need;
-    }
-    if (n > c->cap_idx) {
-        cudaFree(c->d_offsets); cudaFree(c->d_lens); c->d_offsets = nullptr; c->d_lens = nullptr; c->cap_idx = 0;
-        CK(cudaMalloc(&c->d_offsets, sizeof(int64_t) * n));
-        CK(cudaMalloc(&c->d_lens, sizeof(int32_t) * n));
-        c->cap_idx = n;
-    }
+    if (reserve_staging(c, need, n)) return -1;
     // pieces of about piece_bytes, cut at read boundaries (slots in increasing order; otherwise one piece)
     std::vector<int64_t> cuts(1, 0);
     if (monotonic && c->piece_bytes > 0) {
@@ -848,12 +815,7 @@ int fpl_process_fastq_host(fpl_ctx* c, const uint8_t* text, int64_t n_bytes, int
     if (!records || !results) return fail("fpl_process_fastq_host: records/results is null");
     FplIngest& g = c->ingest;
     const int64_t need = FPL_BATCH_BYTES(g.packed_bytes);
-    if (need > c->cap_bytes) {
-        cudaFree(c->d_seq); cudaFree(c->d_qual); c->d_seq = c->d_qual = nullptr; c->cap_bytes = 0;
-        CK(cudaMalloc(&c->d_seq, need));
-        CK(cudaMalloc(&c->d_qual, need));
-        c->cap_bytes = need;
-    }
+    if (reserve_staging(c, need, 0)) return -1;
     // slot padding is never interpreted, but keep it defined for whole-vector reads past a read's end
     CK(cudaMemsetAsync(c->d_seq, 0, need, c->stream));
     CK(cudaMemsetAsync(c->d_qual, 0, need, c->stream));
@@ -886,9 +848,9 @@ int fpl_emit_fastq_host(fpl_ctx* c, int want_failed, uint8_t* out, int64_t out_c
         const bool ext = c->P.opt.mask_enabled || c->P.opt.break_enabled;
         EmitSource src = {};
         src.text = c->ingest.d_text; src.rec = c->ingest.d_rec; src.res = c->last_results; src.n_reads = c->emit_n;
-        src.segs = ext ? c->ext.d_segs : nullptr;
-        src.seg_off = ext ? c->ext.d_off : nullptr;
-        src.mseq = (c->P.opt.mask_enabled && c->ext.n_segs > 0) ? c->ext.d_mseq : nullptr;   // fpl_ext_run made the masked copy
+        src.segs = ext ? c->ext.d_segs.get() : nullptr;
+        src.seg_off = ext ? c->ext.d_off.get() : nullptr;
+        src.mseq = (c->P.opt.mask_enabled && c->ext.n_segs > 0) ? c->ext.d_mseq.get() : nullptr;   // fpl_ext_run made the masked copy
         src.offsets = c->ingest.d_offsets;
         char err[256] = "";
         if (fpl_emit_build(&e, src, want_failed != 0, c->stream, err, sizeof(err))) return fail("fpl_emit_fastq_host: %s", err);
@@ -922,9 +884,9 @@ int fpl_emit_batch_device(fpl_ctx* c, fpl_out_batch* out, fpl_out_batch* failed)
     const bool ext = c->P.opt.mask_enabled || c->P.opt.break_enabled;
     EmitSource src = {};
     src.res = c->last_results; src.n_reads = c->bsrc.n_reads;
-    src.segs = ext ? c->ext.d_segs : nullptr;
-    src.seg_off = ext ? c->ext.d_off : nullptr;
-    src.mseq = (c->P.opt.mask_enabled && c->ext.n_segs > 0) ? c->ext.d_mseq : nullptr;   // fpl_ext_run made the masked copy
+    src.segs = ext ? c->ext.d_segs.get() : nullptr;
+    src.seg_off = ext ? c->ext.d_off.get() : nullptr;
+    src.mseq = (c->P.opt.mask_enabled && c->ext.n_segs > 0) ? c->ext.d_mseq.get() : nullptr;   // fpl_ext_run made the masked copy
     src.offsets = c->bsrc.offsets; src.seq = c->bsrc.seq; src.qual = c->bsrc.qual;
     FplBatchEmit& e = c->bemit;
     if (!e.built) {
@@ -1136,10 +1098,8 @@ int fpl_comm_init(fpl_ctx* c, const uint8_t* id, int rank, int n_ranks) {
     memcpy(&u, id, sizeof(u));
     CKN(nccl().CommInitRank(&c->comm, n_ranks, u, rank));
     c->comm_rank = rank; c->comm_size = n_ranks;
-    if (!c->d_agree) {
-        CK(cudaMalloc(&c->d_agree, sizeof(long long)));
-        CK(cudaMallocHost(&c->h_agree, sizeof(long long)));
-    }
+    CK(c->d_agree.grow_exact(1));
+    if (!c->h_agree) CK(cudaMallocHost(&c->h_agree, sizeof(long long)));
     return 0;
 }
 
@@ -1349,16 +1309,6 @@ std::vector<std::string> report_frame(const fpl_options& o, const std::vector<st
     return p;
 }
 
-int grow_dev(void** ptr, int64_t* cap, int64_t need) {
-    if (need <= *cap) return 0;
-    int64_t n = *cap ? *cap : (1 << 16);
-    while (n < need) n *= 2;
-    cudaFree(*ptr); *ptr = nullptr; *cap = 0;
-    CK(cudaMalloc(ptr, (size_t)n));
-    *cap = n;
-    return 0;
-}
-
 // the text of the accumulators as they are now, into c->rep
 int report_build(fpl_ctx* c, const char* version, const char* command, bool is_rna) {
     FplReport& r = c->rep;
@@ -1366,7 +1316,7 @@ int report_build(fpl_ctx* c, const char* version, const char* command, bool is_r
     const int64_t C = c->C;
     cudaStream_t s = c->stream;
     // 1. total_cycles, bases and G+C of both blocks; the tails and the counters come to the host
-    if (!r.d_sum) CK(cudaMalloc(&r.d_sum, 6 * sizeof(unsigned long long)));
+    CK(r.d_sum.grow_exact(6));
     unsigned long long sum[6] = {(unsigned long long)C, 0, 0, (unsigned long long)C, 0, 0};
     CK(cudaMemcpyAsync(r.d_sum, sum, sizeof(sum), cudaMemcpyHostToDevice, s));
     { Timed t(c, K_REPORT_CYCLES); launch_report_cycles(c->d_stats[0], c->d_stats[1], C, r.d_sum, s); }
@@ -1392,14 +1342,11 @@ int report_build(fpl_ctx* c, const char* version, const char* command, bool is_r
     R.blk[0] = c->d_stats[0]; R.blk[1] = c->d_stats[1]; R.C = C; R.T[0] = b[0].cycles; R.T[1] = b[1].cycles;
     R.is_rna = is_rna ? 1 : 0;
     const int64_t n = 11 * (R.T[0] + R.T[1]);
-    if (grow_dev((void**)&r.d_size, &r.cap_size, (int64_t)sizeof(int64_t) * (n + 1))) return -1;
-    if (grow_dev((void**)&r.d_off, &r.cap_off, (int64_t)sizeof(int64_t) * (n + 1))) return -1;
+    CK(r.d_size.grow(n + 1));
+    CK(r.d_off.grow(n + 1));
     CK(cudaMemsetAsync(r.d_size + n, 0, sizeof(int64_t), s));
     { Timed t(c, K_REPORT_SIZES); launch_report_sizes(R, r.d_size, s); }
-    size_t tb = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, r.d_size, r.d_off, n + 1, s));
-    if (grow_dev(&r.d_tmp, &r.cap_tmp, (int64_t)tb + 256)) return -1;
-    CK(cub::DeviceScan::ExclusiveSum(r.d_tmp, tb, r.d_size, r.d_off, n + 1, s));
+    CK(cub_call(r.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, r.d_size.get(), r.d_off.get(), n + 1, s); }));
     int64_t end[22];                   // the running sum behind curve j
     for (int j = 0; j < 22; j++) {
         const int w = j / 11, k = j % 11;
@@ -1424,12 +1371,12 @@ int report_build(fpl_ctx* c, const char* version, const char* command, bool is_r
     memcpy(r.h_frame.data(), src.data(), sizeof(int64_t) * 24);
     memcpy(r.h_frame.data() + sizeof(int64_t) * 24, dst.data(), sizeof(int64_t) * 23);
     for (int j = 0; j < 23; j++) memcpy(r.h_frame.data() + tables + src[j], frame[j].data(), frame[j].size());
-    if (grow_dev((void**)&r.d_frame, &r.cap_frame, (int64_t)r.h_frame.size())) return -1;
-    if (grow_dev((void**)&r.d_text, &r.cap_text, total)) return -1;
+    CK(r.d_frame.grow((int64_t)r.h_frame.size()));
+    CK(r.d_text.grow(total));
     CK(cudaMemcpyAsync(r.d_frame, r.h_frame.data(), r.h_frame.size(), cudaMemcpyHostToDevice, s));
     {
         Timed t(c, K_REPORT_TEXT);
-        const int64_t* d_src = reinterpret_cast<const int64_t*>(r.d_frame);
+        const int64_t* d_src = reinterpret_cast<const int64_t*>(r.d_frame.get());
         launch_report_text(R, r.d_off, r.d_frame + tables, d_src, d_src + 24, 23, r.d_text, s);
         c->launches++;                 // + k_report_frame
     }
@@ -1825,8 +1772,6 @@ std::vector<std::string> html_frame(const fpl_options& o, const long long* cnt, 
     return p;
 }
 
-template <class T> int grow_t(T** p, int64_t* cap, int64_t n) { return grow_dev((void**)p, cap, (int64_t)sizeof(T) * n); }
-
 int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
     FplHtml& h = c->html;
     FplLists& L = c->lists;
@@ -1834,8 +1779,8 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
     const int64_t C = c->C;
     cudaStream_t s = c->stream;
     // 1. total_cycles, bases and G+C (k_report_cycles), then the base-bin counts below total_cycles
-    if (!h.d_sum) CK(cudaMalloc(&h.d_sum, 22 * sizeof(unsigned long long)));
-    if (!h.d_lstat) CK(cudaMalloc(&h.d_lstat, 8 * sizeof(int)));
+    CK(h.d_sum.grow_exact(22));
+    CK(h.d_lstat.grow_exact(8));
     unsigned long long sum[22] = {(unsigned long long)C, 0, 0, (unsigned long long)C, 0, 0};
     CK(cudaMemcpyAsync(h.d_sum, sum, sizeof(sum), cudaMemcpyHostToDevice, s));
     { Timed t(c, K_HTML_CYCLES); launch_report_cycles(c->d_stats[0], c->d_stats[1], C, h.d_sum, s); }
@@ -1858,13 +1803,12 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
         const int64_t n = L.n[w], nch = (n + HTML_CHUNK - 1) / HTML_CHUNK;
         if (!n) continue;
         const int64_t m = HTML_BINS * nch + 1;
-        if (grow_t(&h.d_mat, &h.cap_mat, m) || grow_t(&h.d_moff, &h.cap_moff, m) || grow_t(&h.d_grp[w], &h.cap_grp[w], n)) return -1;
+        CK(h.d_mat.grow(m));
+        CK(h.d_moff.grow(m));
+        CK(h.d_grp[w].grow(n));
         CK(cudaMemsetAsync(h.d_mat + m - 1, 0, sizeof(long long), s));
         { Timed t(c, K_HTML_GROUP_HIST); launch_html_hist(L.d[w], n, nch, h.d_mat, s); }
-        size_t tb = 0;
-        CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, h.d_mat, h.d_moff, m, s));
-        if (grow_dev(&h.d_tmp, &h.cap_tmp, (int64_t)tb + 256)) return -1;
-        CK(cub::DeviceScan::ExclusiveSum(h.d_tmp, tb, h.d_mat, h.d_moff, m, s));
+        CK(cub_call(h.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, h.d_mat.get(), h.d_moff.get(), m, s); }));
         { Timed t(c, K_HTML_GROUP_SCATTER); launch_html_scatter(L.d[w], n, nch, h.d_moff, h.d_grp[w], s); }
         CK(cudaMemcpyAsync(&NE[w], h.d_moff + 128 * nch, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(&M[w], h.d_moff + 129 * nch, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
@@ -1872,7 +1816,8 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
     }
     // 3. Stats::calcLengthHistogram over [0, longest read]
     const int64_t H = c->used_cycles + 1;
-    if (grow_t(&h.d_hist, &h.cap_hist, 2 * H) || grow_t(&h.d_lwork, &h.cap_lwork, 6 * H)) return -1;
+    CK(h.d_hist.grow(2 * H));
+    CK(h.d_lwork.grow(6 * H));
     CK(cudaMemsetAsync(h.d_hist, 0, sizeof(unsigned long long) * 2 * H, s));
     const int init[8] = {INT_MAX, -1, INT_MAX, INT_MAX, INT_MAX, -1, INT_MAX, INT_MAX};
     CK(cudaMemcpyAsync(h.d_lstat, init, sizeof(init), cudaMemcpyHostToDevice, s));
@@ -1882,14 +1827,8 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
         Timed t(c, K_HTML_LENGTHS);
         launch_html_lenhist(L.d[w], L.n[w], hist, s);
         launch_html_lenprod(hist, H, prod, s);
-        size_t tb = 0;
-        CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, hist, ccum, H, s));
-        if (grow_dev(&h.d_tmp, &h.cap_tmp, (int64_t)tb + 256)) return -1;
-        CK(cub::DeviceScan::ExclusiveSum(h.d_tmp, tb, hist, ccum, H, s));
-        tb = 0;
-        CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, prod, pcum, H, s));
-        if (grow_dev(&h.d_tmp, &h.cap_tmp, (int64_t)tb + 256)) return -1;
-        CK(cub::DeviceScan::ExclusiveSum(h.d_tmp, tb, prod, pcum, H, s));
+        CK(cub_call(h.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, hist, ccum, H, s); }));
+        CK(cub_call(h.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, prod, pcum, H, s); }));
         const long long lensum = tails[w * FPL_STATS_TAIL + FPL_STATS_LENSUM];
         launch_html_lensearch(hist, ccum, prod, pcum, H, lensum / 2, (unsigned long long)M[w] / 2, h.d_lstat + 4 * w, s);
         c->launches += L.n[w] ? 2 : 1;               // k_html_lenhist (with entries), k_html_lenprod, k_html_lensearch
@@ -1917,9 +1856,9 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
     }
     // 4. the per-cycle values, then the down-sampled means
     const int64_t R[2] = {(int64_t)b[0].x.size(), (int64_t)b[1].x.size()};
-    if (grow_t(&h.d_x, &h.cap_x, R[0] + R[1] + 1) || grow_t(&h.d_vals, &h.cap_vals, 11 * (T[0] + T[1]) + 1) ||
-        grow_t(&h.d_sums, &h.cap_sums, 11 * (R[0] + R[1]) + 1))
-        return -1;
+    CK(h.d_x.grow(R[0] + R[1] + 1));
+    CK(h.d_vals.grow(11 * (T[0] + T[1]) + 1));
+    CK(h.d_sums.grow(11 * (R[0] + R[1]) + 1));
     std::vector<long long> xs(b[0].x);
     xs.insert(xs.end(), b[1].x.begin(), b[1].x.end());
     if (!xs.empty()) CK(cudaMemcpyAsync(h.d_x, xs.data(), sizeof(long long) * xs.size(), cudaMemcpyHostToDevice, s));
@@ -1953,13 +1892,11 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
         X.sums[w] = h.d_sums + (w ? 11 * R[0] : 0);
         X.x[w] = h.d_x + (w ? R[0] : 0);
     }
-    if (grow_t(&h.d_size, &h.cap_size, items + 1) || grow_t(&h.d_off, &h.cap_off, items + 1)) return -1;
+    CK(h.d_size.grow(items + 1));
+    CK(h.d_off.grow(items + 1));
     CK(cudaMemsetAsync(h.d_size + items, 0, sizeof(int64_t), s));
     if (items) { Timed t(c, K_HTML_SIZES); launch_html_sizes(X, h.d_size, s); }
-    size_t tb = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, h.d_size, h.d_off, items + 1, s));
-    if (grow_dev(&h.d_tmp, &h.cap_tmp, (int64_t)tb + 256)) return -1;
-    CK(cub::DeviceScan::ExclusiveSum(h.d_tmp, tb, h.d_size, h.d_off, items + 1, s));
+    CK(cub_call(h.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, h.d_size.get(), h.d_off.get(), items + 1, s); }));
     int64_t end[HTML_SEGS];            // the running sum behind segment j
     for (int j = 0; j < HTML_SEGS; j++)
         CK(cudaMemcpyAsync(&end[j], h.d_off + X.start[j + 1], sizeof(int64_t), cudaMemcpyDeviceToHost, s));
@@ -1982,11 +1919,12 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
     memcpy(h.h_frame.data(), src.data(), sizeof(int64_t) * (np + 1));
     memcpy(h.h_frame.data() + sizeof(int64_t) * (np + 1), dst.data(), sizeof(int64_t) * np);
     for (int j = 0; j < np; j++) memcpy(h.h_frame.data() + tables + src[j], frame[j].data(), frame[j].size());
-    if (grow_t(&h.d_frame, &h.cap_frame, (int64_t)h.h_frame.size()) || grow_t(&h.d_text, &h.cap_text, total)) return -1;
+    CK(h.d_frame.grow((int64_t)h.h_frame.size()));
+    CK(h.d_text.grow(total));
     CK(cudaMemcpyAsync(h.d_frame, h.h_frame.data(), h.h_frame.size(), cudaMemcpyHostToDevice, s));
     {
         Timed t(c, K_HTML_TEXT);
-        const int64_t* d_src = reinterpret_cast<const int64_t*>(h.d_frame);
+        const int64_t* d_src = reinterpret_cast<const int64_t*>(h.d_frame.get());
         launch_html_text(X, h.d_off, h.d_frame + tables, d_src, d_src + np + 1, np, h.d_text, s);
         if (items) c->launches++;      // k_report_frame + k_html_text (only with values to print)
     }
@@ -2078,7 +2016,7 @@ extern "C" int fpl_merge_stats(fpl_ctx* c, fpl_ctx* const* src, int n_src) {
     // the capacities first: they synchronise dst's stream when they grow
     if (reserve_cycles(c, rows)) return -1;
     if (L.keep && (grow_list(c, 0, total[0]) || grow_list(c, 1, total[1]))) return -1;
-    if (grow_t(&c->d_merge, &c->cap_merge, n_src)) return -1;
+    CK(c->d_merge.grow(n_src));
     if (!c->merge_ev) CK(cudaEventCreateWithFlags(&c->merge_ev, cudaEventDisableTiming));
     for (int k = 0; k < n_src; k++) {         // behind everything queued on the sources
         CK(cudaEventRecord(c->merge_ev, src[k]->stream));

@@ -259,57 +259,37 @@ k_emit_batch_copy(const EmitSource S, const int64_t* __restrict__ off, const Emi
 
 }  // namespace
 
-#define CKM(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { snprintf(err, errlen, "%s failed: %s", #call, cudaGetErrorString(e_)); return -1; } } while (0)
-
-static int growm(void** p, int64_t* cap, int64_t need, char* err, size_t errlen) {
-    if (need <= *cap) return 0;
-    int64_t c = *cap ? *cap : (1 << 16);
-    while (c < need) c *= 2;
-    cudaFree(*p); *p = nullptr; *cap = 0;
-    CKM(cudaMalloc(p, (size_t)c));
-    *cap = c;
-    return 0;
-}
-
 int fpl_emit_build(FplEmit* e, const EmitSource& src, bool want_failed, cudaStream_t s, char* err, size_t errlen) {
     e->built = false; e->out_bytes = e->failed_bytes = 0; e->with_failed = want_failed;
     const int64_t n = src.n_reads;
     if (n == 0) { e->built = true; return 0; }
     const int64_t m = 2 * n + 2;
-    if (growm((void**)&e->d_size, &e->cap_size, (int64_t)sizeof(int64_t) * m, err, errlen)) return -1;
-    if (growm((void**)&e->d_off, &e->cap_off, (int64_t)sizeof(int64_t) * m, err, errlen)) return -1;
-    CKM(cudaMemsetAsync(e->d_size + n, 0, sizeof(int64_t), s));
-    CKM(cudaMemsetAsync(e->d_size + 2 * n + 1, 0, sizeof(int64_t), s));
+    FPL_CK_ERR(e->d_size.grow(m));
+    FPL_CK_ERR(e->d_off.grow(m));
+    FPL_CK_ERR(cudaMemsetAsync(e->d_size + n, 0, sizeof(int64_t), s));
+    FPL_CK_ERR(cudaMemsetAsync(e->d_size + 2 * n + 1, 0, sizeof(int64_t), s));
     k_emit_sizes<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src, want_failed, e->d_size);
-    size_t tb = 0;
-    CKM(cub::DeviceScan::ExclusiveSum(nullptr, tb, e->d_size, e->d_off, m, s));
-    if (growm(&e->d_tmp, &e->cap_tmp, (int64_t)tb + 256, err, errlen)) return -1;
-    CKM(cub::DeviceScan::ExclusiveSum(e->d_tmp, tb, e->d_size, e->d_off, m, s));
+    FPL_CK_ERR(cub_call(e->d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, e->d_size.get(), e->d_off.get(), m, s); }));
     int64_t total_out = 0, total_both = 0;
-    CKM(cudaMemcpyAsync(&total_out, e->d_off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-    CKM(cudaMemcpyAsync(&total_both, e->d_off + 2 * n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-    CKM(cudaStreamSynchronize(s));
+    FPL_CK_ERR(cudaMemcpyAsync(&total_out, e->d_off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    FPL_CK_ERR(cudaMemcpyAsync(&total_both, e->d_off + 2 * n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    FPL_CK_ERR(cudaStreamSynchronize(s));
     e->out_bytes = total_out;
     e->failed_bytes = total_both - total_out;
     // + 16: a warp's last 16-byte store never needs a bounds test against the next buffer
-    if (growm((void**)&e->d_out, &e->cap_out, e->out_bytes + 16, err, errlen)) return -1;
-    if (growm((void**)&e->d_failed, &e->cap_failed, e->failed_bytes + 16, err, errlen)) return -1;
+    FPL_CK_ERR(e->d_out.grow(e->out_bytes + 16));
+    FPL_CK_ERR(e->d_failed.grow(e->failed_bytes + 16));
     const int64_t want = (n + 7) / 8;
     k_emit_copy<<<(unsigned)(want < FPL_NUM_SMS * 16 ? want : FPL_NUM_SMS * 16), 256, 0, s>>>(src, want_failed, e->d_off, e->d_out, e->d_failed);
-    CKM(cudaGetLastError());
+    FPL_CK_ERR(cudaGetLastError());
     e->built = true;
     return 0;
 }
 
-void fpl_emit_free(FplEmit* e) {
-    cudaFree(e->d_size); cudaFree(e->d_off); cudaFree(e->d_out); cudaFree(e->d_failed); cudaFree(e->d_tmp);
-    *e = FplEmit();
-}
-
 int fpl_emit_batch_reserve(FplBatchEmit* e, int64_t n_reads, char* err, size_t errlen) {
     const int64_t m = 4 * (n_reads + 1);
-    if (growm((void**)&e->d_cnt, &e->cap_cnt, (int64_t)sizeof(int64_t) * m, err, errlen)) return -1;
-    if (growm((void**)&e->d_off, &e->cap_off, (int64_t)sizeof(int64_t) * m, err, errlen)) return -1;
+    FPL_CK_ERR(e->d_cnt.grow(m));
+    FPL_CK_ERR(e->d_off.grow(m));
     return 0;
 }
 
@@ -319,13 +299,10 @@ void launch_emit_batch_sizes(const EmitSource& src, int64_t* cnt, cudaStream_t s
 
 int fpl_emit_batch_scan(FplBatchEmit* e, int64_t n_reads, cudaStream_t s, char* err, size_t errlen) {
     const int64_t q = n_reads + 1, m = 4 * q;
-    size_t tb = 0;
-    CKM(cub::DeviceScan::ExclusiveSum(nullptr, tb, e->d_cnt, e->d_off, m, s));
-    if (growm(&e->d_tmp, &e->cap_tmp, (int64_t)tb + 256, err, errlen)) return -1;
-    CKM(cub::DeviceScan::ExclusiveSum(e->d_tmp, tb, e->d_cnt, e->d_off, m, s));
+    FPL_CK_ERR(cub_call(e->d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, e->d_cnt.get(), e->d_off.get(), m, s); }));
     int64_t end[4] = {0, 0, 0, 0};    // running sum at the end of each vector (its entry n is 0, so that is the next one's start)
-    for (int i = 0; i < 4; i++) CKM(cudaMemcpyAsync(&end[i], e->d_off + (i + 1) * q - 1, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-    CKM(cudaStreamSynchronize(s));
+    for (int i = 0; i < 4; i++) FPL_CK_ERR(cudaMemcpyAsync(&end[i], e->d_off + (i + 1) * q - 1, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    FPL_CK_ERR(cudaStreamSynchronize(s));
     e->n_out = end[0]; e->out_bytes = end[1] - end[0]; e->n_failed = end[2] - end[1]; e->failed_bytes = end[3] - end[2];
     return 0;
 }
@@ -334,9 +311,4 @@ void launch_emit_batch_copy(const EmitSource& src, const int64_t* off, const Emi
                             cudaStream_t s) {
     const int64_t want = (src.n_reads + 7) / 8;
     k_emit_batch_copy<<<(unsigned)(want < FPL_NUM_SMS * 16 ? want : FPL_NUM_SMS * 16), 256, 0, s>>>(src, off, out, failed);
-}
-
-void fpl_emit_batch_free(FplBatchEmit* e) {
-    cudaFree(e->d_cnt); cudaFree(e->d_off); cudaFree(e->d_tmp);
-    *e = FplBatchEmit();
 }

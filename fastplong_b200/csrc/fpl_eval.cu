@@ -9,6 +9,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include "fplgpu.h"
+#include "fpl_buf.h"
 
 namespace {
 constexpr int KEYLEN = 10;
@@ -56,31 +57,27 @@ extern "C" int fpl_eval_adapter_kmers(int device, const fpl_batch* b, int32_t sh
     if (!b || !counts || !position_acc || !total || side < 0 || side > 1 || shift_tail < 0 || b->n_reads < 0) return -1;
     if (cudaSetDevice(device) != cudaSuccess) return -2;
     const size_t size = (size_t)1 << (2 * KEYLEN);
-    uint8_t* d_seq = nullptr; int64_t* d_off = nullptr; int32_t* d_len = nullptr;
-    unsigned int* d_cnt = nullptr; unsigned long long* d_acc = nullptr; unsigned long long* d_tot = nullptr;
-    int rc = 0;
+    DevBuf<uint8_t> d_seq; DevBuf<int64_t> d_off; DevBuf<int32_t> d_len;
+    DevBuf<unsigned int> d_cnt; DevBuf<unsigned long long> d_acc, d_tot;
     const int64_t n = b->n_reads;
     // only the two ends of every read are looked at, but the packed layout is uploaded as it is (64 Ki reads at most)
-    if (cudaMalloc(&d_seq, (size_t)b->n_bytes + 64) != cudaSuccess || cudaMalloc(&d_off, sizeof(int64_t) * (n + 1)) != cudaSuccess ||
-        cudaMalloc(&d_len, sizeof(int32_t) * (n + 1)) != cudaSuccess || cudaMalloc(&d_cnt, sizeof(unsigned int) * size) != cudaSuccess ||
-        cudaMalloc(&d_acc, sizeof(unsigned long long) * size) != cudaSuccess || cudaMalloc(&d_tot, sizeof(unsigned long long)) != cudaSuccess)
-        rc = -3;
-    if (!rc) {
-        cudaMemcpy(d_seq, b->seq, (size_t)b->n_bytes, cudaMemcpyHostToDevice);
-        cudaMemcpy(d_off, b->offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice);
-        cudaMemcpy(d_len, b->lens, sizeof(int32_t) * n, cudaMemcpyHostToDevice);
-        cudaMemset(d_cnt, 0, sizeof(unsigned int) * size);
-        cudaMemset(d_acc, 0, sizeof(unsigned long long) * size);
-        cudaMemset(d_tot, 0, sizeof(unsigned long long));
-        if (n) k_eval_kmers<<<(unsigned)((n * 32 + 255) / 256), 256>>>(d_seq, d_off, d_len, n, shift_tail, side, d_cnt, d_acc, d_tot);
-        unsigned long long t = 0;
-        if (cudaMemcpy(counts, d_cnt, sizeof(unsigned int) * size, cudaMemcpyDeviceToHost) != cudaSuccess ||
-            cudaMemcpy(position_acc, d_acc, sizeof(unsigned long long) * size, cudaMemcpyDeviceToHost) != cudaSuccess ||
-            cudaMemcpy(&t, d_tot, sizeof(t), cudaMemcpyDeviceToHost) != cudaSuccess)
-            rc = -4;
-        *total = (int64_t)t;
-    }
-    cudaFree(d_seq); cudaFree(d_off); cudaFree(d_len); cudaFree(d_cnt); cudaFree(d_acc); cudaFree(d_tot);
+    if (d_seq.grow_exact(b->n_bytes + 64) || d_off.grow_exact(n + 1) || d_len.grow_exact(n + 1) || d_cnt.grow_exact(size) ||
+        d_acc.grow_exact(size) || d_tot.grow_exact(1))
+        return -3;
+    cudaMemcpy(d_seq, b->seq, (size_t)b->n_bytes, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_off, b->offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_len, b->lens, sizeof(int32_t) * n, cudaMemcpyHostToDevice);
+    cudaMemset(d_cnt, 0, sizeof(unsigned int) * size);
+    cudaMemset(d_acc, 0, sizeof(unsigned long long) * size);
+    cudaMemset(d_tot, 0, sizeof(unsigned long long));
+    if (n) k_eval_kmers<<<(unsigned)((n * 32 + 255) / 256), 256>>>(d_seq, d_off, d_len, n, shift_tail, side, d_cnt, d_acc, d_tot);
+    unsigned long long t = 0;
+    int rc = 0;
+    if (cudaMemcpy(counts, d_cnt, sizeof(unsigned int) * size, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(position_acc, d_acc, sizeof(unsigned long long) * size, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(&t, d_tot, sizeof(t), cudaMemcpyDeviceToHost) != cudaSuccess)
+        rc = -4;
+    *total = (int64_t)t;
     return rc;
 }
 

@@ -273,26 +273,6 @@ __global__ void k_ext_fill_records(int64_t n_reads, const int32_t* __restrict__ 
     }
 }
 
-#define CKE(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { snprintf(err, errlen, "%s failed: %s", #call, cudaGetErrorString(e_)); return -1; } } while (0)
-
-static int growb(void** p, int64_t* cap, int64_t need, char* err, size_t errlen) {
-    if (need <= *cap) return 0;
-    int64_t c = *cap ? *cap : (1 << 16);
-    while (c < need) c *= 2;
-    cudaFree(*p); *p = nullptr; *cap = 0;
-    CKE(cudaMalloc(p, (size_t)c));
-    *cap = c;
-    return 0;
-}
-
-static int scan_i32(FplExt* x, int32_t* in, int32_t* out, int64_t n, cudaStream_t s, char* err, size_t errlen) {
-    size_t tb = 0;
-    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n, s));
-    if (growb(&x->d_tmp, &x->cap_tmp, (int64_t)tb + 256, err, errlen)) return -1;
-    CKE(cub::DeviceScan::ExclusiveSum(x->d_tmp, tb, in, out, n, s));
-    return 0;
-}
-
 // Runs after k_final (which left the initial segments in the records).  Returns the sequence buffer the post-filter
 // Stats must read (the masked copy when --mask is on) through *fseq_out, and the StatSeg list in x->d_stat.
 int fpl_ext_run(FplExt* x, const DevParams& P, const DevBatch& b, int64_t n_bytes, fpl_read_result* res,
@@ -303,35 +283,35 @@ int fpl_ext_run(FplExt* x, const DevParams& P, const DevBatch& b, int64_t n_byte
     *fseq_out = b.seq;
     if (n == 0) return 0;
     if (2 * n + 1 >= (1ll << 31)) { snprintf(err, errlen, "too many reads for --mask/--break in one call"); return -1; }
-    if (growb((void**)&x->d_cnt, &x->cap_cnt, (int64_t)sizeof(int32_t) * (2 * n + 1), err, errlen)) return -1;
-    if (growb((void**)&x->d_off, &x->cap_off, (int64_t)sizeof(int32_t) * (2 * n + 1), err, errlen)) return -1;
+    FPL_CK_ERR(x->d_cnt.grow(2 * n + 1));
+    FPL_CK_ERR(x->d_off.grow(2 * n + 1));
     const unsigned g2 = (unsigned)((2 * n + 255) / 256);
     k_ext_count<<<g2, 256, 0, s>>>(P, b, res, x->d_cnt);
-    CKE(cudaMemsetAsync(x->d_cnt + 2 * n, 0, sizeof(int32_t), s));
-    if (scan_i32(x, x->d_cnt, x->d_off, 2 * n + 1, s, err, errlen)) return -1;
+    FPL_CK_ERR(cudaMemsetAsync(x->d_cnt + 2 * n, 0, sizeof(int32_t), s));
+    FPL_CK_ERR(cub_call(x->d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, x->d_cnt.get(), x->d_off.get(), 2 * n + 1, s); }));
     int32_t total = 0;
-    CKE(cudaMemcpyAsync(&total, x->d_off + 2 * n, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    CKE(cudaStreamSynchronize(s));
+    FPL_CK_ERR(cudaMemcpyAsync(&total, x->d_off + 2 * n, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    FPL_CK_ERR(cudaStreamSynchronize(s));
     x->n_segs = total;
-    if (growb((void**)&x->d_segs, &x->cap_segs, (int64_t)sizeof(fpl_segment) * (total + 1), err, errlen)) return -1;
-    if (growb((void**)&x->d_stat, &x->cap_stat, (int64_t)sizeof(StatSeg) * (total + 1), err, errlen)) return -1;
+    FPL_CK_ERR(x->d_segs.grow((int64_t)total + 1));
+    FPL_CK_ERR(x->d_stat.grow((int64_t)total + 1));
     k_ext_emit<<<g2, 256, 0, s>>>(P, b, res, x->d_off, x->d_segs);
     if (P.opt.mask_enabled && total > 0) {
         // the masked copy is a batch of its own: its tail pad is defined, not whatever the buffer held before
-        if (growb((void**)&x->d_mseq, &x->cap_mseq, FPL_BATCH_BYTES(n_bytes), err, errlen)) return -1;
-        CKE(cudaMemcpyAsync(x->d_mseq, b.seq, (size_t)n_bytes, cudaMemcpyDeviceToDevice, s));
-        CKE(cudaMemsetAsync(x->d_mseq + n_bytes, 0, (size_t)(FPL_BATCH_BYTES(n_bytes) - n_bytes), s));
-        if (growb((void**)&x->d_rcnt, &x->cap_rcnt, (int64_t)sizeof(int32_t) * (total + 1), err, errlen)) return -1;
-        if (growb((void**)&x->d_roff, &x->cap_roff, (int64_t)sizeof(int32_t) * (total + 1), err, errlen)) return -1;
+        FPL_CK_ERR(x->d_mseq.grow(FPL_BATCH_BYTES(n_bytes)));
+        FPL_CK_ERR(cudaMemcpyAsync(x->d_mseq, b.seq, (size_t)n_bytes, cudaMemcpyDeviceToDevice, s));
+        FPL_CK_ERR(cudaMemsetAsync(x->d_mseq + n_bytes, 0, (size_t)(FPL_BATCH_BYTES(n_bytes) - n_bytes), s));
+        FPL_CK_ERR(x->d_rcnt.grow((int64_t)total + 1));
+        FPL_CK_ERR(x->d_roff.grow((int64_t)total + 1));
         const unsigned gs = (unsigned)((total + 255) / 256);
         k_ext_mask_count<<<gs, 256, 0, s>>>(P, b, x->d_segs, total, x->d_rcnt);
-        CKE(cudaMemsetAsync(x->d_rcnt + total, 0, sizeof(int32_t), s));
-        if (scan_i32(x, x->d_rcnt, x->d_roff, (int64_t)total + 1, s, err, errlen)) return -1;
+        FPL_CK_ERR(cudaMemsetAsync(x->d_rcnt + total, 0, sizeof(int32_t), s));
+        FPL_CK_ERR(cub_call(x->d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, x->d_rcnt.get(), x->d_roff.get(), (int64_t)total + 1, s); }));
         int32_t nreg = 0;
-        CKE(cudaMemcpyAsync(&nreg, x->d_roff + total, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-        CKE(cudaStreamSynchronize(s));
+        FPL_CK_ERR(cudaMemcpyAsync(&nreg, x->d_roff + total, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+        FPL_CK_ERR(cudaStreamSynchronize(s));
         x->n_regs = nreg;
-        if (growb((void**)&x->d_regs, &x->cap_regs, (int64_t)sizeof(fpl_region) * (nreg + 1), err, errlen)) return -1;
+        FPL_CK_ERR(x->d_regs.grow((int64_t)nreg + 1));
         k_ext_mask_emit<<<gs, 256, 0, s>>>(P, b, x->d_segs, total, x->d_roff, x->d_regs, x->d_mseq);
         *fseq_out = x->d_mseq;
     }
@@ -342,12 +322,6 @@ int fpl_ext_run(FplExt* x, const DevParams& P, const DevBatch& b, int64_t n_byte
                                                                                       stats_post, C, x->d_segs);
     }
     k_ext_fill_records<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(n, x->d_off, x->d_segs, res);
-    CKE(cudaGetLastError());
+    FPL_CK_ERR(cudaGetLastError());
     return 0;
-}
-
-void fpl_ext_free(FplExt* x) {
-    cudaFree(x->d_cnt); cudaFree(x->d_off); cudaFree(x->d_segs); cudaFree(x->d_stat); cudaFree(x->d_rcnt);
-    cudaFree(x->d_roff); cudaFree(x->d_regs); cudaFree(x->d_mseq); cudaFree(x->d_tmp);
-    *x = FplExt();
 }

@@ -96,65 +96,51 @@ k_fastq_pack(const uint8_t* __restrict__ text, const fpl_fastq_record* __restric
 
 }  // namespace
 
-#define CKI(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { snprintf(err, errlen, "%s failed: %s", #call, cudaGetErrorString(e_)); return -1; } } while (0)
-
-static int grow(void** p, int64_t* cap, int64_t need, char* err, size_t errlen) {
-    if (need <= *cap) return 0;
-    int64_t c = *cap ? *cap : (1 << 20);
-    while (c < need) c *= 2;
-    cudaFree(*p); *p = nullptr; *cap = 0;
-    CKI(cudaMalloc(p, (size_t)c));
-    *cap = c;
-    return 0;
-}
-
 int fpl_ingest_index(FplIngest* g, const uint8_t* h_text, int64_t n, int is_last, cudaStream_t s, int64_t* n_records,
                      int64_t* consumed, char* err, size_t errlen) {
     *n_records = 0; *consumed = 0;
     if (n == 0) return 0;
-    if (grow((void**)&g->d_text, &g->cap_text, n + 64, err, errlen)) return -1;
-    CKI(cudaMemcpyAsync(g->d_text, h_text, (size_t)n, cudaMemcpyHostToDevice, s));
-    CKI(cudaMemsetAsync(g->d_text + n, 0, 64, s));
+    FPL_CK_ERR(g->d_text.grow(n + 64, FPL_INGEST_FIRST_BYTES));
+    FPL_CK_ERR(cudaMemcpyAsync(g->d_text, h_text, (size_t)n, cudaMemcpyHostToDevice, s));
+    FPL_CK_ERR(cudaMemsetAsync(g->d_text + n, 0, 64, s));
     // misc: [0] newline count, [1] count written by cub, [2] first bad record, [4] CR flag
-    if (!g->d_misc) CKI(cudaMalloc((void**)&g->d_misc, 64));
-    CKI(cudaMemsetAsync(g->d_misc, 0, 64, s));
-    CKI(cudaMemsetAsync(g->d_misc + 2, 0xFF, 8, s));   // first_bad = ~0
-    k_count_lines<<<(unsigned)((n + 16 * 256 - 1) / (16 * 256)), 256, 0, s>>>(g->d_text, n, (unsigned long long*)g->d_misc);
+    FPL_CK_ERR(g->d_misc.grow_exact(8));
+    FPL_CK_ERR(cudaMemsetAsync(g->d_misc, 0, 64, s));
+    FPL_CK_ERR(cudaMemsetAsync(g->d_misc + 2, 0xFF, 8, s));   // first_bad = ~0
+    k_count_lines<<<(unsigned)((n + 16 * 256 - 1) / (16 * 256)), 256, 0, s>>>(g->d_text, n, g->d_misc);
     struct { int64_t n_nl; int has_cr; int pad; } h;
-    CKI(cudaMemcpyAsync(&h.n_nl, g->d_misc, 8, cudaMemcpyDeviceToHost, s));
-    CKI(cudaMemcpyAsync(&h.has_cr, g->d_misc + 4, 4, cudaMemcpyDeviceToHost, s));
-    CKI(cudaStreamSynchronize(s));
+    FPL_CK_ERR(cudaMemcpyAsync(&h.n_nl, g->d_misc, 8, cudaMemcpyDeviceToHost, s));
+    FPL_CK_ERR(cudaMemcpyAsync(&h.has_cr, g->d_misc + 4, 4, cudaMemcpyDeviceToHost, s));
+    FPL_CK_ERR(cudaStreamSynchronize(s));
     if (h.has_cr) return 1;   // CR line ends: the reference's getLine() has its own rules for them
     g->n_nl = h.n_nl;
-    if (grow((void**)&g->d_nl, &g->cap_nl, (int64_t)sizeof(int64_t) * (h.n_nl + 1), err, errlen)) return -1;
+    FPL_CK_ERR(g->d_nl.grow(h.n_nl + 1, FPL_INGEST_FIRST_BYTES));
     cub::CountingInputIterator<int64_t> idx(0);
     IsNewline pred{g->d_text};
-    size_t tb = 0;
-    CKI(cub::DeviceSelect::If(nullptr, tb, idx, g->d_nl, (int64_t*)(g->d_misc + 1), n, pred, s));
-    if (grow(&g->d_tmp, &g->cap_tmp, (int64_t)tb + 256, err, errlen)) return -1;
-    CKI(cub::DeviceSelect::If(g->d_tmp, tb, idx, g->d_nl, (int64_t*)(g->d_misc + 1), n, pred, s));
+    FPL_CK_ERR(cub_call(g->d_tmp, [&](void* t, size_t& b) {
+        return cub::DeviceSelect::If(t, b, idx, g->d_nl.get(), (int64_t*)(g->d_misc + 1), n, pred, s);
+    }, FPL_INGEST_FIRST_BYTES));
     // complete lines: every newline ends one; at the end of the input an unterminated last line counts too
     uint8_t lastc = h_text[n - 1];
     int64_t n_lines = h.n_nl + ((is_last && lastc != '\n') ? 1 : 0);
     const int64_t nrec = n_lines / 4;
     if (is_last && n_lines % 4 != 0) return 1;        // trailing partial record / blank lines: let the reference decide
     if (nrec == 0) return 0;
-    if (grow((void**)&g->d_rec, &g->cap_rec, (int64_t)sizeof(fpl_fastq_record) * nrec, err, errlen)) return -1;
-    if (grow((void**)&g->d_lens, &g->cap_lens, (int64_t)sizeof(int32_t) * nrec, err, errlen)) return -1;
-    if (grow((void**)&g->d_slots, &g->cap_slots, (int64_t)sizeof(int64_t) * (nrec + 1), err, errlen)) return -1;
-    if (grow((void**)&g->d_offsets, &g->cap_offsets, (int64_t)sizeof(int64_t) * (nrec + 1), err, errlen)) return -1;
+    FPL_CK_ERR(g->d_rec.grow(nrec, FPL_INGEST_FIRST_BYTES));
+    FPL_CK_ERR(g->d_lens.grow(nrec, FPL_INGEST_FIRST_BYTES));
+    FPL_CK_ERR(g->d_slots.grow(nrec + 1, FPL_INGEST_FIRST_BYTES));
+    FPL_CK_ERR(g->d_offsets.grow(nrec + 1, FPL_INGEST_FIRST_BYTES));
     k_fastq_records<<<(unsigned)((nrec + 255) / 256), 256, 0, s>>>(g->d_text, n, g->d_nl, h.n_nl, nrec, g->d_rec, g->d_lens,
-                                                                  g->d_slots, (unsigned long long*)(g->d_misc + 2));
-    CKI(cudaMemsetAsync(g->d_slots + nrec, 0, 8, s));
-    tb = 0;
-    CKI(cub::DeviceScan::ExclusiveSum(nullptr, tb, g->d_slots, g->d_offsets, nrec + 1, s));
-    if (grow(&g->d_tmp, &g->cap_tmp, (int64_t)tb + 256, err, errlen)) return -1;
-    CKI(cub::DeviceScan::ExclusiveSum(g->d_tmp, tb, g->d_slots, g->d_offsets, nrec + 1, s));
+                                                                  g->d_slots, g->d_misc + 2);
+    FPL_CK_ERR(cudaMemsetAsync(g->d_slots + nrec, 0, 8, s));
+    FPL_CK_ERR(cub_call(g->d_tmp, [&](void* t, size_t& b) {
+        return cub::DeviceScan::ExclusiveSum(t, b, g->d_slots.get(), g->d_offsets.get(), nrec + 1, s);
+    }, FPL_INGEST_FIRST_BYTES));
     unsigned long long first_bad = 0;
     int64_t total = 0;
-    CKI(cudaMemcpyAsync(&first_bad, g->d_misc + 2, 8, cudaMemcpyDeviceToHost, s));
-    CKI(cudaMemcpyAsync(&total, g->d_offsets + nrec, 8, cudaMemcpyDeviceToHost, s));
-    CKI(cudaStreamSynchronize(s));
+    FPL_CK_ERR(cudaMemcpyAsync(&first_bad, g->d_misc + 2, 8, cudaMemcpyDeviceToHost, s));
+    FPL_CK_ERR(cudaMemcpyAsync(&total, g->d_offsets + nrec, 8, cudaMemcpyDeviceToHost, s));
+    FPL_CK_ERR(cudaStreamSynchronize(s));
     if (first_bad != ~0ull) return 1;   // a record the strict layout does not describe
     g->packed_bytes = total;
     *n_records = nrec;
@@ -162,7 +148,7 @@ int fpl_ingest_index(FplIngest* g, const uint8_t* h_text, int64_t n, int is_last
     int64_t last_nl_idx = 4 * nrec - 1;
     if (last_nl_idx < h.n_nl) {
         int64_t pos = 0;
-        CKI(cudaMemcpy(&pos, g->d_nl + last_nl_idx, 8, cudaMemcpyDeviceToHost));
+        FPL_CK_ERR(cudaMemcpy(&pos, g->d_nl + last_nl_idx, 8, cudaMemcpyDeviceToHost));
         *consumed = pos + 1;
     } else {
         *consumed = n;
@@ -174,12 +160,6 @@ int fpl_ingest_pack(FplIngest* g, int64_t nrec, uint8_t* d_seq, uint8_t* d_qual,
     if (nrec == 0) return 0;
     const int64_t want = (nrec + 7) / 8;
     k_fastq_pack<<<(unsigned)(want < FPL_NUM_SMS * 32 ? want : FPL_NUM_SMS * 32), 256, 0, s>>>(g->d_text, g->d_rec, g->d_offsets, nrec, d_seq, d_qual);
-    CKI(cudaGetLastError());
+    FPL_CK_ERR(cudaGetLastError());
     return 0;
-}
-
-void fpl_ingest_free(FplIngest* g) {
-    cudaFree(g->d_text); cudaFree(g->d_nl); cudaFree(g->d_rec); cudaFree(g->d_lens); cudaFree(g->d_slots);
-    cudaFree(g->d_offsets); cudaFree(g->d_tmp); cudaFree(g->d_misc);
-    *g = FplIngest();
 }

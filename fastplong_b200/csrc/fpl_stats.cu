@@ -636,11 +636,6 @@ __global__ void k_cs_gather(const StatSeg* __restrict__ segs, const uint32_t* __
 }
 }  // namespace
 
-void fpl_cycle_ws_free(CycleWs* ws) {
-    cudaFree(ws->tmp); cudaFree(ws->k_in); cudaFree(ws->k_out); cudaFree(ws->v_in); cudaFree(ws->v_out); cudaFree(ws->sorted);
-    *ws = CycleWs();
-}
-
 // kmer_also: where the 5-mer counts of this launch go besides `stats` (nullptr = nowhere else); do_kmer = false skips
 // them.  fused_post (with do_kmer, segs = the pre-filter list, one per read): the post-filter list; the segments
 // cs_fused_takes accepts are counted into stats_post by the same pass.  residual_of (segs = that post-filter list): the
@@ -669,36 +664,31 @@ int launch_cycle_stats(CycleWs* ws, const uint8_t* seq, const uint8_t* qual, con
     int end_bit = 1;
     while (end_bit < 31 && (max_len >> end_bit)) end_bit++;
     size_t need = 0;
-    cub::DeviceRadixSort::SortPairsDescending(nullptr, need, ws->k_in, ws->k_out, ws->v_in, ws->v_out, (int)nseg, 0, end_bit, stream);
-    if (nseg > ws->cap || need > ws->tmp_bytes) {
+    cub::DeviceRadixSort::SortPairsDescending(nullptr, need, ws->k_in.get(), ws->k_out.get(), ws->v_in.get(), ws->v_out.get(), (int)nseg, 0,
+                                              end_bit, stream);
+    if (nseg > ws->cap || (int64_t)need > ws->tmp.bytes()) {
         cudaStreamSynchronize(stream);
-        const int64_t cap = nseg > ws->cap ? nseg : ws->cap;
-        void* tmp = ws->tmp; size_t tmp_bytes = ws->tmp_bytes;
         if (nseg > ws->cap) {
-            cudaFree(ws->k_in); cudaFree(ws->k_out); cudaFree(ws->v_in); cudaFree(ws->v_out); cudaFree(ws->sorted);
-            ws->k_in = ws->k_out = nullptr; ws->v_in = ws->v_out = nullptr; ws->sorted = nullptr; ws->cap = 0;
-            if (cudaMalloc(&ws->k_in, 4 * cap) != cudaSuccess || cudaMalloc(&ws->k_out, 4 * cap) != cudaSuccess ||
-                cudaMalloc(&ws->v_in, 4 * cap) != cudaSuccess || cudaMalloc(&ws->v_out, 4 * cap) != cudaSuccess ||
-                cudaMalloc(&ws->sorted, sizeof(SegD) * cap) != cudaSuccess)
+            ws->cap = 0;
+            if (ws->k_in.grow_exact(nseg) || ws->k_out.grow_exact(nseg) || ws->v_in.grow_exact(nseg) || ws->v_out.grow_exact(nseg) ||
+                ws->sorted.grow_exact(nseg))
                 return -1;
-            ws->cap = cap;
+            ws->cap = nseg;
             // the temporary storage grows with the item count
-            cub::DeviceRadixSort::SortPairsDescending(nullptr, need, ws->k_in, ws->k_out, ws->v_in, ws->v_out, (int)cap, 0, 31, stream);
+            cub::DeviceRadixSort::SortPairsDescending(nullptr, need, ws->k_in.get(), ws->k_out.get(), ws->v_in.get(), ws->v_out.get(),
+                                                      (int)nseg, 0, 31, stream);
         }
-        if (need > tmp_bytes) {
-            cudaFree(tmp); ws->tmp = nullptr; ws->tmp_bytes = 0;
-            if (cudaMalloc(&ws->tmp, need) != cudaSuccess) return -1;
-            ws->tmp_bytes = need;
-        }
+        if (ws->tmp.grow_exact((int64_t)need)) return -1;
     }
     const unsigned blocks = (unsigned)((nseg + 255) / 256);
     k_cs_keys<<<blocks, 256, 0, stream>>>(segs, nseg, ws->k_in, ws->v_in, residual_of);
-    size_t bytes = ws->tmp_bytes;
-    cub::DeviceRadixSort::SortPairsDescending(ws->tmp, bytes, ws->k_in, ws->k_out, ws->v_in, ws->v_out, (int)nseg, 0, end_bit, stream);
+    size_t bytes = (size_t)ws->tmp.bytes();
+    cub::DeviceRadixSort::SortPairsDescending(ws->tmp.get(), bytes, ws->k_in.get(), ws->k_out.get(), ws->v_in.get(), ws->v_out.get(), (int)nseg,
+                                              0, end_bit, stream);
     const bool fuse = do_kmer && fused_post != nullptr;
-    k_cs_gather<<<blocks, 256, 0, stream>>>(segs, ws->k_out, ws->v_out, nseg, static_cast<SegD*>(ws->sorted), fuse ? fused_post : nullptr);
+    k_cs_gather<<<blocks, 256, 0, stream>>>(segs, ws->k_out, ws->v_out, nseg, ws->sorted, fuse ? fused_post : nullptr);
     dim3 grid((unsigned)((max_len + 15 + CS_TILE - 1) / CS_TILE), (unsigned)((nseg + CS_GROUP - 1) / CS_GROUP));
-    const SegD* sorted = static_cast<const SegD*>(ws->sorted);
+    const SegD* sorted = ws->sorted;
     const int al = aligned ? 1 : 0;
     static const bool tma = getenv("FPL_CS_TMA") != nullptr && atoi(getenv("FPL_CS_TMA")) != 0;
     if (tma) {

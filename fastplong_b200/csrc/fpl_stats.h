@@ -3,15 +3,16 @@
 #include <cstddef>
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "fpl_buf.h"
 
+struct SegD;
 struct CycleWs {
-    void* tmp = nullptr; size_t tmp_bytes = 0;
-    uint32_t *k_in = nullptr, *k_out = nullptr;
-    int32_t *v_in = nullptr, *v_out = nullptr;
-    void* sorted = nullptr;
-    int64_t cap = 0;
+    DevBuf<uint8_t> tmp;
+    DevBuf<uint32_t> k_in, k_out;
+    DevBuf<int32_t> v_in, v_out;
+    DevBuf<SegD> sorted;
+    int64_t cap = 0;                    // segments every list above holds
 };
-void fpl_cycle_ws_free(CycleWs* ws);
 
 // fpl_report_json: the two Stats blocks whose curves k_report_sizes / k_report_text print
 struct ReportCurves {

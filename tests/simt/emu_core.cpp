@@ -40,6 +40,10 @@ void bulk(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
 }  // namespace emu
 extern "C" void emu_set_cp_async_lazy(int on) { emu::cp_lazy = on; }
 extern "C" long long emu_collectives() { return emu::collectives; }
+namespace emu { long long live_allocs = 0, fail_alloc_in = 0; }      // fake/cuda_runtime.h: emu_alloc
+extern "C" long long emu_live_allocs() { return emu::live_allocs; }
+// -> the count it replaces: > 0 when the allocation it was set for never came
+extern "C" long long emu_fail_alloc(long long k) { const long long was = emu::fail_alloc_in; emu::fail_alloc_in = k; return was; }
 extern "C" long long emu_blocks() { return (long long)emu::block_serial; }
 
 // ---------------- NVRTC + driver: kernels "compiled" for the host ----------------

@@ -4,7 +4,7 @@
 #include "../emu_cuda.h"
 #include <time.h>
 
-enum cudaError_t { cudaSuccess = 0, cudaErrorInvalidValue = 1, cudaErrorNotReady = 600 };
+enum cudaError_t { cudaSuccess = 0, cudaErrorInvalidValue = 1, cudaErrorMemoryAllocation = 2, cudaErrorNotReady = 600 };
 enum cudaMemcpyKind { cudaMemcpyHostToHost = 0, cudaMemcpyHostToDevice = 1, cudaMemcpyDeviceToHost = 2, cudaMemcpyDeviceToDevice = 3, cudaMemcpyDefault = 4 };
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2, cudaFuncAttributeMaxDynamicSharedMemorySize = 8 };
 struct EmuEvent { double t; };
@@ -16,17 +16,20 @@ static inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 static inline cudaError_t cudaSetDevice(int d) { return d == 0 ? cudaSuccess : cudaErrorInvalidValue; }
 static inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }
 // cudaMalloc does not zero memory: EMU_MALLOC_FILL=<byte> fills every allocation with that byte (default 0), so that a kernel or
-// host path leaning on fresh allocations being zero shows up
+// host path leaning on fresh allocations being zero shows up.  emu::live_allocs counts the cudaMalloc / cudaMallocHost blocks not
+// yet freed; emu::fail_alloc_in = k > 0 makes the k-th allocation from now fail, once (emu_core.cpp: emu_live_allocs, emu_fail_alloc).
+namespace emu { extern long long live_allocs, fail_alloc_in; }
 static inline void* emu_alloc(size_t n) {
+    if (emu::fail_alloc_in > 0 && --emu::fail_alloc_in == 0) return nullptr;
     static const char* f = getenv("EMU_MALLOC_FILL");
     void* p = malloc(n ? n : 1);
-    if (p) memset(p, f ? (int)strtol(f, nullptr, 0) : 0, n ? n : 1);
+    if (p) { memset(p, f ? (int)strtol(f, nullptr, 0) : 0, n ? n : 1); emu::live_allocs++; }
     return p;
 }
-template <class T> static inline cudaError_t cudaMalloc(T** p, size_t n) { *p = (T*)emu_alloc(n); return *p ? cudaSuccess : cudaErrorInvalidValue; }
-template <class T> static inline cudaError_t cudaMallocHost(T** p, size_t n) { *p = (T*)emu_alloc(n); return *p ? cudaSuccess : cudaErrorInvalidValue; }
-static inline cudaError_t cudaFree(void* p) { free(p); return cudaSuccess; }
-static inline cudaError_t cudaFreeHost(void* p) { free(p); return cudaSuccess; }
+template <class T> static inline cudaError_t cudaMalloc(T** p, size_t n) { *p = (T*)emu_alloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
+template <class T> static inline cudaError_t cudaMallocHost(T** p, size_t n) { *p = (T*)emu_alloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
+static inline cudaError_t cudaFree(void* p) { if (p) { emu::live_allocs--; free(p); } return cudaSuccess; }
+static inline cudaError_t cudaFreeHost(void* p) { if (p) { emu::live_allocs--; free(p); } return cudaSuccess; }
 static inline cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { if (n) memmove(d, s, n); return cudaSuccess; }
 static inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t = nullptr) { if (n) memmove(d, s, n); return cudaSuccess; }
 static inline cudaError_t cudaMemcpy2DAsync(void* d, size_t dpitch, const void* s, size_t spitch, size_t width, size_t height, cudaMemcpyKind,

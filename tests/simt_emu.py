@@ -185,10 +185,14 @@ def build_binary():
 
 # ---- binding.Engine on the emulated library ----
 def emulated_library():
-    """ctypes handle of the emulated library (emulator switches: emu_set_cp_async_lazy, emu_collectives, emu_blocks)"""
+    """ctypes handle of the emulated library (emulator switches: emu_set_cp_async_lazy, emu_collectives, emu_blocks; emu_live_allocs:
+    cudaMalloc / cudaMallocHost blocks not yet freed; emu_fail_alloc(k): the k-th allocation from now fails, once, 0 = none; it
+    returns the count it replaces, > 0 when that allocation never came)"""
     lib = C.CDLL(build_library())
     lib.emu_set_cp_async_lazy.argtypes = [C.c_int]
-    lib.emu_collectives.restype = lib.emu_blocks.restype = C.c_longlong
+    lib.emu_collectives.restype = lib.emu_blocks.restype = lib.emu_live_allocs.restype = C.c_longlong
+    lib.emu_fail_alloc.argtypes = [C.c_longlong]
+    lib.emu_fail_alloc.restype = C.c_longlong
     return lib
 
 

@@ -1,0 +1,175 @@
+"""Who owns the library's device memory, on the emulated library (tests/simt_emu.py), whose cudaMalloc / cudaMallocHost count the
+blocks alive (emu_live_allocs) and fail the k-th allocation from now on request (emu_fail_alloc).  A context frees everything its
+entry points allocated when it is destroyed; an allocation that fails anywhere in a call makes the call fail and leaks nothing;
+fpl_stats_reserve is all or nothing; a report or emit build that failed gives the same bytes when it is called again."""
+import gc
+
+import numpy as np
+import pytest
+
+import cases
+import simt_emu
+from fastplong_b200 import abi, synth
+from fastplong_b200.binding import FplError
+
+PLAIN, EXT = cases.OPTION_SETS["cut_polyx_cplx"], cases.MASK_BREAK_SETS["mask_and_break"]
+BATCH = cases.blocky_quality_batch(5, n=12)
+TEXT = b"".join(b"@r%d\n%s\n+\n%s\n" % (i, *BATCH.read(i)) for i in range(BATCH.n_reads))
+
+
+@pytest.fixture(scope="module")
+def lib():
+    return simt_emu.emulated_library()
+
+
+def engine(opt):
+    e = simt_emu.EmuEngine(opt)
+    e.keep_read_lists()
+    return e
+
+
+def process_device(e, batch):
+    """fpl_process_device on copies of the batch that the engine keeps (device memory is host memory here)"""
+    size = abi.batch_bytes(batch.n_bytes)
+    e.dev = [np.zeros(size, np.uint8), np.zeros(size, np.uint8), batch.offsets.astype(np.int64), batch.lens.astype(np.int32)]
+    e.dev[0][:batch.n_bytes], e.dev[1][:batch.n_bytes] = batch.seq, batch.qual
+    e.process_device(*(a.ctypes.data for a in e.dev), batch.n_reads, batch.n_bytes)
+
+
+def emit_batch(e):
+    return [bytes(t.numpy()) for b in e.emit_batch(True, device="cpu") for t in (b.seq, b.qual, b.offsets, b.lens, b.segs)]
+
+
+def with_source(e):
+    """e and e.src, another context with the same options, have processed a batch: fpl_merge_stats(e, [e.src]) is ready"""
+    e.process(BATCH)
+    e.src = engine(e.options)
+    e.src.process(BATCH)
+
+
+def close(e):
+    for x in (e, getattr(e, "src", None)):
+        if x:
+            x.close()
+
+
+# entry point -> (what the context has done before, the call); the calls marked True are retried after a failure
+ENTRIES = {
+    "fpl_process_host": (None, lambda e: e.process(BATCH), False),
+    "fpl_process_device": (None, lambda e: process_device(e, BATCH), False),
+    "fpl_process_fastq_host": (None, lambda e: e.process_fastq(TEXT), False),
+    "fpl_emit_fastq_host": (lambda e: e.process_fastq(TEXT), lambda e: e.emit_fastq(True), True),
+    "fpl_emit_batch_device": (lambda e: e.process(BATCH), emit_batch, True),
+    "fpl_report_json": (lambda e: e.process(BATCH), lambda e: e.report_json(command="fastplong -i x"), True),
+    "fpl_report_html": (lambda e: e.process(BATCH), lambda e: e.report_html(command="fastplong -i x", time_text="t"), True),
+    "fpl_merge_stats": (with_source, lambda e: e.merge(e.src), False),
+    "fpl_stats_reserve": (lambda e: e.process(BATCH), lambda e: e.reserve_cycles(1 << 14), False),
+}
+
+
+def live(lib):
+    gc.collect()
+    return lib.emu_live_allocs()
+
+
+@pytest.mark.parametrize("opt", [PLAIN, EXT], ids=["plain", "mask_break"])
+def test_a_context_frees_everything_it_allocated(lib, opt):
+    base = live(lib)
+    e = engine(opt)
+    e.process(BATCH)
+    e.emit_batch(True, device="cpu")
+    process_device(e, BATCH)
+    e.emit_batch(True, device="cpu")
+    e.process_fastq(TEXT)
+    e.emit_fastq(True)
+    e.emit_batch(True, device="cpu")
+    e.report_json()
+    e.report_html(time_text="t")
+    src = engine(opt)
+    src.process(BATCH)
+    e.merge(src)
+    e.report_html(time_text="t")
+    e.reset()
+    e.process(synth.ont_like(4, 3000, 11))      # longer than the first capacity: the Stats blocks grow
+    e.close()
+    src.close()
+    assert live(lib) == base
+
+
+@pytest.mark.parametrize("opt", [PLAIN, EXT], ids=["plain", "mask_break"])
+def test_a_failed_fpl_create_leaks_nothing(lib, opt):
+    base, k = live(lib), 0
+    while True:
+        k += 1
+        lib.emu_fail_alloc(k)
+        try:
+            engine(opt).close()
+            failed = False
+        except FplError:
+            failed = True
+        pending = lib.emu_fail_alloc(0)
+        assert live(lib) == base, f"allocation {k} failed: leak"
+        if pending:
+            assert not failed and k > 1
+            return
+        assert failed, f"allocation {k} failed, fpl_create succeeded"
+
+
+@pytest.mark.parametrize("entry", list(ENTRIES))
+@pytest.mark.parametrize("opt", [PLAIN, EXT], ids=["plain", "mask_break"])
+def test_an_allocation_failure_leaks_nothing(lib, opt, entry):
+    """every allocation the call makes fails once in turn: the call fails and leaks nothing; a report or emit call made again
+    gives what a context that never failed gives"""
+    before, call, retry = ENTRIES[entry]
+    want = None
+    if retry:
+        e = engine(opt)
+        before(e)
+        want = call(e)
+        close(e)
+    base, k = live(lib), 0
+    while True:
+        k += 1
+        e = engine(opt)
+        if before:
+            before(e)
+        lib.emu_fail_alloc(k)
+        try:
+            call(e)
+            failed = False
+        except FplError:
+            failed = True
+        pending = lib.emu_fail_alloc(0)
+        if pending:
+            assert not failed and k > 1, f"{entry} allocates nothing here"
+        else:
+            assert failed, f"{entry}: allocation {k} failed, the call succeeded"
+            if retry:
+                assert call(e) == want, f"{entry} retried after allocation {k} failed"
+        close(e)
+        assert live(lib) == base, f"{entry}: allocation {k} failed: leak"
+        if pending:
+            return
+
+
+def test_a_failed_fpl_stats_reserve_changes_nothing(lib):
+    e, fresh = engine(PLAIN), engine(PLAIN)
+    for x in (e, fresh):
+        x.process(BATCH)
+    cycles, stats = e.cycles, [e.stats(w) for w in (0, 1)]
+    lib.emu_fail_alloc(2)                    # the second of the two new blocks
+    with pytest.raises(FplError):
+        e.reserve_cycles(4 * cycles)
+    assert lib.emu_fail_alloc(0) == 0
+    assert e.cycles == cycles
+    for w in (0, 1):
+        np.testing.assert_array_equal(e.stats(w), stats[w])
+    longer = synth.ont_like(4, 3000, 11)      # longer than the capacity: the blocks grow and take the rows along
+    for x in (e, fresh):
+        x.process(longer)
+    assert e.cycles == fresh.cycles > cycles
+    for w in (0, 1):
+        np.testing.assert_array_equal(e.stats(w), fresh.stats(w))
+    np.testing.assert_array_equal(e.counters(), fresh.counters())
+    e.close()
+    fresh.close()
