@@ -143,9 +143,17 @@ struct FplReport {
     int64_t n_bytes = 0;
 };
 
+// the context's NCCL communicator, released by ncclCommDestroy (defined where nccl() is)
+struct CommRelease { void operator()(ncclComm_t m) const; };
+
+// The owners of the streams come first: they go last, after everything that work queued on them uses.  fpl_destroy
+// synchronises both streams before the context goes.
 struct fpl_ctx {
     int device = 0;
-    cudaStream_t stream = nullptr;
+    Stream stream;
+    // fpl_process_host: the upload runs on its own stream, piece by piece, and the kernels of a piece start as soon
+    // as its bytes have arrived (copy/compute overlap inside one call)
+    Stream copy_stream;
     DevParams P;
     ScanPlan plan;
     FplJitKernel jit;   // specialised scan kernel (NVRTC), fn == nullptr if not used
@@ -198,30 +206,28 @@ struct fpl_ctx {
     std::vector<int32_t> h_lens;
     // tiling + measurement
     int64_t tile_bases = 0;
-    // fpl_process_host: the upload runs on its own stream, piece by piece, and the kernels of a piece start as soon
-    // as its bytes have arrived (copy/compute overlap inside one call)
-    cudaStream_t copy_stream = nullptr;
     DevBuf<int> d_minmax;               // fpl_process_device: min / max read length of the batch
-    int* h_minmax = nullptr;
-    std::vector<cudaEvent_t> piece_events;
+    PinnedHost<int> h_minmax;
+    std::vector<Event> piece_events;
     int64_t piece_bytes = 16ll << 20;
     bool timing = false;
     float kernel_ms[K_NKERNELS];
     int64_t kernel_n[K_NKERNELS];
     int64_t launches = 0;
     // multi-GPU merge (fpl_comm_init / fpl_allreduce_stats): one NCCL communicator per context
-    ncclComm_t comm = nullptr;
+    Owned<ncclComm_t, CommRelease> comm;
     int comm_rank = 0, comm_size = 1;
     int64_t used_cycles = 0;            // longest read accumulated since the last fpl_reset
     int64_t reduced_rows = 0;           // widest fpl_allreduce_stats since then: other ranks' reads may fill rows past used_cycles
     DevBuf<long long> d_agree;          // device word for the all-reduce(max) of the cycle count
-    long long* h_agree = nullptr;       // pinned
+    PinnedHost<long long> h_agree;
     // fpl_merge_stats: the sources' table (k_merge_stats) and the event that orders the streams
     DevBuf<MergeSrc> d_merge;
-    cudaEvent_t merge_ev = nullptr;
-    struct Ev { int k; cudaEvent_t a, b; };
+    Event merge_ev;
+    // timing (Timed): the recorded start / end pairs not yet collected, and the collected events for reuse
+    struct Ev { int k; Event a, b; };
     std::vector<Ev> events;
-    std::vector<cudaEvent_t> pool;
+    std::vector<Event> pool;
 };
 
 static int ensure_reads(fpl_ctx* c, int64_t n) {
@@ -281,21 +287,25 @@ static int reserve_staging(fpl_ctx* c, int64_t n_bytes, int64_t n_reads) {
     return 0;
 }
 
-static cudaEvent_t get_event(fpl_ctx* c) {
-    if (!c->pool.empty()) { cudaEvent_t e = c->pool.back(); c->pool.pop_back(); return e; }
-    cudaEvent_t e;
-    cudaEventCreate(&e);
+// a timing event from the pool, or a new one; empty when none can be created
+static Event get_event(fpl_ctx* c) {
+    Event e;
+    if (c->pool.empty()) { create_event(e, true); return e; }
+    e = std::move(c->pool.back());
+    c->pool.pop_back();
     return e;
 }
 
+// A launch timed when timing is on and both its events exist; without them it runs untimed.  It is counted either way.
 struct Timed {
-    fpl_ctx* c; int k; bool ours; cudaEvent_t a = nullptr, b = nullptr;
+    fpl_ctx* c; int k; bool ours; Event a, b;
     Timed(fpl_ctx* c_, int k_, bool ours_ = true) : c(c_), k(k_), ours(ours_) {   // ours = false: a library kernel (NCCL), timed but not counted
-        if (c->timing) { a = get_event(c); b = get_event(c); cudaEventRecord(a, c->stream); }
+        if (c->timing) { a = get_event(c); b = get_event(c); }
+        if (a && b) cudaEventRecord(a, c->stream);
     }
     ~Timed() {
         if (ours) c->launches++;
-        if (c->timing) { cudaEventRecord(b, c->stream); c->events.push_back({k, a, b}); }
+        if (a && b) { cudaEventRecord(b, c->stream); c->events.push_back({k, std::move(a), std::move(b)}); }
     }
 };
 
@@ -304,10 +314,10 @@ struct Timed {
 static void collect_times(fpl_ctx* c) {
     size_t keep = 0;
     for (auto& e : c->events) {
-        if (cudaEventQuery(e.b) != cudaSuccess) { c->events[keep++] = e; continue; }
+        if (cudaEventQuery(e.b) != cudaSuccess) { c->events[keep++] = std::move(e); continue; }
         float ms = 0;
         if (cudaEventElapsedTime(&ms, e.a, e.b) == cudaSuccess) { c->kernel_ms[e.k] += ms; c->kernel_n[e.k]++; }
-        c->pool.push_back(e.a); c->pool.push_back(e.b);
+        c->pool.push_back(std::move(e.a)); c->pool.push_back(std::move(e.b));
     }
     c->events.resize(keep);
 }
@@ -332,7 +342,7 @@ __global__ void k_lens_minmax(const int32_t* __restrict__ lens, const int64_t* _
 // h_lens may be null when the caller knows the longest read (known_max_len >= 0) and nothing below needs the individual
 // lengths (no tiling, no pieces): a device-resident batch then never waits for the host to walk a million lengths.
 static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fpl_read_result* d_res_out, int64_t n_bytes,
-                     const std::vector<int64_t>* cuts = nullptr, const cudaEvent_t* arrived = nullptr,
+                     const std::vector<int64_t>* cuts = nullptr, const Event* arrived = nullptr,
                      int64_t known_max_len = -1) {
     const int64_t n = full.n_reads;
     CK(cudaSetDevice(c->device));
@@ -503,7 +513,7 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
     CK(cudaSetDevice(opt->device));
     CK(cudaDeviceSynchronize());        // the first call that needs the device context creates it
     stamp("driver + device context");
-    fpl_ctx* c = new fpl_ctx();
+    std::unique_ptr<fpl_ctx> c(new fpl_ctx());     // released to the caller on success, freed on every failure
     c->device = opt->device;
     c->n_adapters = n;
     // host tables
@@ -524,10 +534,8 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
         const char* s = k == 0 ? ad->start : k == 1 ? ad->end : ad->fasta[k - 2];
         if (!s) s = "";
         size_t len = strlen(s);
-        if (len > FPL_MAX_ADAPTER_LEN) {
-            delete c;
+        if (len > FPL_MAX_ADAPTER_LEN)
             return fail("fpl_create: adapter %d is %zu bp, longer than FPL_MAX_ADAPTER_LEN=%d", k, len, FPL_MAX_ADAPTER_LEN);
-        }
         h_alen[k] = (int)len;
         c->adapter_str.push_back(s);
         memcpy(&h_ad[(size_t)k * FPL_MAX_ADAPTER_LEN], s, len);
@@ -589,21 +597,20 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
         c->plan.halo_words = ((maxa - 1) >> 5) + 1;
     }
     for (int i = 0; i <= FPL_MAX_ADAPTER_LEN; i++) c->P.thr[i] = (short)(int)round(opt->ed_max * i);  // src/adaptertrimmer.cpp:73
-#define CKC(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { fail("%s failed: %s", #call, cudaGetErrorString(e_)); fpl_destroy(c); return -1; } } while (0)
-    CKC(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    CKC(c->d_adapters.grow_exact((int64_t)h_ad.size()));
-    CKC(c->d_alen.grow_exact(n));
-    CKC(c->d_peq.grow_exact((int64_t)h_peq.size()));
-    CKC(c->d_peq16.grow_exact((int64_t)h_peq16.size()));
-    CKC(c->d_acode.grow_exact((int64_t)h_acode.size()));
-    CKC(cudaMemcpy(c->d_acode, h_acode.data(), sizeof(uint32_t) * h_acode.size(), cudaMemcpyHostToDevice));
-    CKC(cudaMemcpy(c->d_adapters, h_ad.data(), h_ad.size(), cudaMemcpyHostToDevice));
-    CKC(cudaMemcpy(c->d_alen, h_alen.data(), sizeof(int) * n, cudaMemcpyHostToDevice));
-    CKC(cudaMemcpy(c->d_peq, h_peq.data(), sizeof(uint4) * h_peq.size(), cudaMemcpyHostToDevice));
-    CKC(cudaMemcpy(c->d_peq16, h_peq16.data(), sizeof(uint32_t) * h_peq16.size(), cudaMemcpyHostToDevice));
+    CK(create_stream(c->stream));
+    CK(c->d_adapters.grow_exact((int64_t)h_ad.size()));
+    CK(c->d_alen.grow_exact(n));
+    CK(c->d_peq.grow_exact((int64_t)h_peq.size()));
+    CK(c->d_peq16.grow_exact((int64_t)h_peq16.size()));
+    CK(c->d_acode.grow_exact((int64_t)h_acode.size()));
+    CK(cudaMemcpy(c->d_acode, h_acode.data(), sizeof(uint32_t) * h_acode.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(c->d_adapters, h_ad.data(), h_ad.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(c->d_alen, h_alen.data(), sizeof(int) * n, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(c->d_peq, h_peq.data(), sizeof(uint4) * h_peq.size(), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(c->d_peq16, h_peq16.data(), sizeof(uint32_t) * h_peq16.size(), cudaMemcpyHostToDevice));
     if (peq_words) {
-        CKC(c->d_peq_long.grow_exact((int64_t)h_peq_long.size()));
-        CKC(cudaMemcpy(c->d_peq_long, h_peq_long.data(), sizeof(unsigned long long) * h_peq_long.size(), cudaMemcpyHostToDevice));
+        CK(c->d_peq_long.grow_exact((int64_t)h_peq_long.size()));
+        CK(cudaMemcpy(c->d_peq_long, h_peq_long.data(), sizeof(unsigned long long) * h_peq_long.size(), cudaMemcpyHostToDevice));
     }
     c->P.peq_long = c->d_peq_long; c->P.peq_words = peq_words;
     if (n > 2) {
@@ -615,14 +622,14 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
                 const int kc = h_alen[k] <= 32 ? 0 : h_alen[k] <= 64 ? 1 : 2;
                 if (kc == cls) order.push_back(k);
             }
-        CKC(c->d_pf_order.grow_exact((int64_t)order.size()));
-        CKC(cudaMemcpy(c->d_pf_order, order.data(), sizeof(int) * order.size(), cudaMemcpyHostToDevice));
+        CK(c->d_pf_order.grow_exact((int64_t)order.size()));
+        CK(cudaMemcpy(c->d_pf_order, order.data(), sizeof(int) * order.size(), cudaMemcpyHostToDevice));
     }
     c->P.pf_order = c->d_pf_order;
     c->P.adapters = c->d_adapters; c->P.alen = c->d_alen; c->P.peq = c->d_peq; c->P.peq16 = c->d_peq16; c->P.acode = c->d_acode;
     c->counter_words = FPL_COUNTER_WORDS(n);
-    CKC(c->d_counters.grow_exact(c->counter_words));
-    CKC(cudaMemset(c->d_counters, 0, sizeof(unsigned long long) * c->counter_words));
+    CK(c->d_counters.grow_exact(c->counter_words));
+    CK(cudaMemset(c->d_counters, 0, sizeof(unsigned long long) * c->counter_words));
     stamp("tables");
     // specialise the scan kernel on the adapters (NVRTC); FPL_NO_JIT=1 keeps the precompiled k_scan_fast
     if (c->plan.fast && getenv("FPL_NO_JIT") == nullptr) {
@@ -640,8 +647,8 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
         }
     }
     if (c->jit.qhist) {
-        CKC(c->d_qstripes.grow_exact(QH_STRIPES * 256));
-        CKC(c->d_nexc.grow_exact(1));
+        CK(c->d_qstripes.grow_exact(QH_STRIPES * 256));
+        CK(c->d_nexc.grow_exact(1));
         c->P.qstripes = c->d_qstripes;
     }
     stamp("scan kernel specialisation");
@@ -653,28 +660,20 @@ int fpl_create(const fpl_options* opt, const fpl_adapters* ad, fpl_ctx** out) {
     const char* pm = getenv("FPL_PIECE_MB");
     if (pm) c->piece_bytes = atoll(pm) > 0 ? atoll(pm) << 20 : 0;
     for (int k = 0; k < K_NKERNELS; k++) { c->kernel_ms[k] = 0; c->kernel_n[k] = 0; }
-    if (reserve_cycles(c, 1024)) { fpl_destroy(c); return -1; }
-    CKC(cudaStreamSynchronize(c->stream));
+    if (reserve_cycles(c.get(), 1024)) return -1;
+    CK(cudaStreamSynchronize(c->stream));
     stamp("accumulators");
-#undef CKC
-    *out = c;
+    *out = c.release();
     return 0;
 }
 
 void fpl_destroy(fpl_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
+    cudaStreamSynchronize(c->stream);
+    if (c->copy_stream) cudaStreamSynchronize(c->copy_stream);
     collect_times(c);
-    for (auto e : c->pool) cudaEventDestroy(e);
-    if (c->merge_ev) cudaEventDestroy(c->merge_ev);
-    for (auto e : c->piece_events) cudaEventDestroy(e);
-    if (c->h_minmax) cudaFreeHost(c->h_minmax);
-    fpl_comm_destroy(c);
-    if (c->h_agree) cudaFreeHost(c->h_agree);
-    if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;                           // the device buffers go with their owners
+    delete c;                           // every resource goes with its owner
 }
 
 int fpl_process_device(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results_dev) {
@@ -688,9 +687,9 @@ int fpl_process_device(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results_
     // the extremes of the lengths (Stats capacity, grid sizes) and the alignment of the offsets are all the host needs
     // to know: reduce them on the side stream, which does not wait for the kernels of the previous batch still running
     // on the compute stream
-    if (!c->copy_stream) CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+    if (!c->copy_stream) CK(create_stream(c->copy_stream));
     CK(c->d_minmax.grow_exact(4));
-    if (!c->h_minmax) CK(cudaMallocHost(&c->h_minmax, 4 * sizeof(int)));
+    if (!c->h_minmax) CK(create_pinned(c->h_minmax, 4));
     c->h_minmax[0] = 0; c->h_minmax[1] = 0; c->h_minmax[2] = 0;
     if (n) {
         const int init[3] = {INT_MAX, INT_MIN, 0};
@@ -755,11 +754,11 @@ int fpl_process_host(fpl_ctx* c, const fpl_batch* b, fpl_read_result* results) {
     }
     cuts.push_back(n);
     const size_t np = cuts.size() - 1;
-    if (!c->copy_stream) CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+    if (!c->copy_stream) CK(create_stream(c->copy_stream));
     while (c->piece_events.size() < np) {
-        cudaEvent_t e;
-        CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        c->piece_events.push_back(e);
+        Event e;
+        CK(create_event(e, false));
+        c->piece_events.push_back(std::move(e));
     }
     // every call ends with a synchronize of the compute stream, so the device buffers are free to overwrite here
     cudaStream_t cs = c->copy_stream;
@@ -1068,6 +1067,8 @@ struct Nccl {
 Nccl& nccl() { static Nccl n; return n; }
 }  // namespace
 
+void CommRelease::operator()(ncclComm_t m) const { nccl().CommDestroy(m); }
+
 #define CKN(call)                                                                                        \
     do {                                                                                                 \
         ncclResult_t r_ = (call);                                                                        \
@@ -1096,10 +1097,12 @@ int fpl_comm_init(fpl_ctx* c, const uint8_t* id, int rank, int n_ranks) {
     CK(cudaSetDevice(c->device));
     ncclUniqueId u;
     memcpy(&u, id, sizeof(u));
-    CKN(nccl().CommInitRank(&c->comm, n_ranks, u, rank));
+    ncclComm_t m = nullptr;
+    CKN(nccl().CommInitRank(&m, n_ranks, u, rank));
+    c->comm.reset(m);
     c->comm_rank = rank; c->comm_size = n_ranks;
     CK(c->d_agree.grow_exact(1));
-    if (!c->h_agree) CK(cudaMallocHost(&c->h_agree, sizeof(long long)));
+    if (!c->h_agree) CK(create_pinned(c->h_agree, 1));
     return 0;
 }
 
@@ -1107,8 +1110,8 @@ int fpl_comm_destroy(fpl_ctx* c) {
     if (!c || !c->comm) return 0;
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
-    nccl().CommDestroy(c->comm);
-    c->comm = nullptr; c->comm_size = 1; c->comm_rank = 0;
+    c->comm.reset();
+    c->comm_size = 1; c->comm_rank = 0;
     return 0;
 }
 
@@ -2017,7 +2020,7 @@ extern "C" int fpl_merge_stats(fpl_ctx* c, fpl_ctx* const* src, int n_src) {
     if (reserve_cycles(c, rows)) return -1;
     if (L.keep && (grow_list(c, 0, total[0]) || grow_list(c, 1, total[1]))) return -1;
     CK(c->d_merge.grow(n_src));
-    if (!c->merge_ev) CK(cudaEventCreateWithFlags(&c->merge_ev, cudaEventDisableTiming));
+    if (!c->merge_ev) CK(create_event(c->merge_ev, false));
     for (int k = 0; k < n_src; k++) {         // behind everything queued on the sources
         CK(cudaEventRecord(c->merge_ev, src[k]->stream));
         CK(cudaStreamWaitEvent(c->stream, c->merge_ev, 0));

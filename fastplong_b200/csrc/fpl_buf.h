@@ -1,11 +1,13 @@
-// Ownership of device memory for the host side of the library: DevBuf<T> owns one cudaMalloc allocation and frees it when it
+// Ownership of CUDA resources for the host side of the library: DevBuf<T> owns one cudaMalloc allocation and frees it when it
 // goes, and its growth methods are the library's only allocation policies.  Kernels and the by-value descriptors (DevBatch,
 // EmitSource, ReportCurves, HtmlText, MergeSrc) take the raw pointer.  Growth returns the CUDA error, so each module keeps
-// its own way of reporting it.
+// its own way of reporting it.  Streams, events and pinned host blocks have owners of their own (Owned, at the end).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <memory>
+#include <type_traits>
 #include <utility>
 
 // a CUDA call in a function that reports into the caller's (err, errlen) buffer
@@ -85,5 +87,41 @@ cudaError_t cub_call(DevBuf<uint8_t>& tmp, F&& call, int64_t first_bytes = FPL_F
     cudaError_t e = call(nullptr, bytes);
     if (e == cudaSuccess) e = tmp.grow((int64_t)bytes + 256, first_bytes);
     if (e == cudaSuccess) e = call(tmp.get(), bytes);
+    return e;
+}
+
+// A unique_ptr whose deleter releases the handle H, handed to CUDA calls as the raw handle (as DevBuf hands out its pointer).
+// The create_* calls below give an owner its handle only when the creation succeeded.
+template <class H, class Release>
+struct Owned : std::unique_ptr<std::remove_pointer_t<H>, Release> {
+    operator H() const { return this->get(); }
+};
+struct StreamRelease { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+struct EventRelease { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+struct PinnedRelease { void operator()(void* p) const { cudaFreeHost(p); } };
+using Stream = Owned<cudaStream_t, StreamRelease>;
+using Event = Owned<cudaEvent_t, EventRelease>;
+template <class T> using PinnedHost = Owned<T*, PinnedRelease>;
+
+// a non-blocking stream
+inline cudaError_t create_stream(Stream& s) {
+    cudaStream_t h;
+    cudaError_t e = cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking);
+    if (e == cudaSuccess) s.reset(h);
+    return e;
+}
+// timing: an event cudaEventElapsedTime can read; otherwise one that only orders work (cudaEventDisableTiming)
+inline cudaError_t create_event(Event& ev, bool timing) {
+    cudaEvent_t h;
+    cudaError_t e = timing ? cudaEventCreate(&h) : cudaEventCreateWithFlags(&h, cudaEventDisableTiming);
+    if (e == cudaSuccess) ev.reset(h);
+    return e;
+}
+// n elements of pinned host memory
+template <class T>
+cudaError_t create_pinned(PinnedHost<T>& p, size_t n) {
+    T* h;
+    cudaError_t e = cudaMallocHost(&h, sizeof(T) * n);
+    if (e == cudaSuccess) p.reset(h);
     return e;
 }

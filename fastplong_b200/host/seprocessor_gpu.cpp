@@ -52,17 +52,25 @@ template <typename T>
 struct Pinned {
     T* p = nullptr;
     size_t cap = 0;
+    Pinned() = default;
+    Pinned(const Pinned&) = delete;
+    Pinned& operator=(const Pinned&) = delete;
+    ~Pinned() { if (p) cudaFreeHost(p); }
     // page-locking is slow (tens of ms per call): grow rarely, never shrink
     void reserve(size_t n, size_t at_least = 0) {
         if (n <= cap) return;
         size_t want = cap ? cap : (at_least ? at_least : 1024);
         while (want < n) want *= 2;
-        T* q = nullptr;
-        if (cudaMallocHost((void**)&q, want * sizeof(T)) != cudaSuccess) error_exit("fastplong_gpu: cudaMallocHost failed");
-        if (p) cudaFreeHost(p);
-        p = q; cap = want;
+        resize(want);
     }
-    ~Pinned() { if (p) cudaFreeHost(p); }
+    // exactly n elements, the first `keep` kept
+    void resize(size_t n, size_t keep = 0) {
+        T* q = nullptr;
+        if (cudaMallocHost((void**)&q, n * sizeof(T)) != cudaSuccess) error_exit("fastplong_gpu: cudaMallocHost failed");
+        if (keep) memcpy(q, p, keep * sizeof(T));
+        if (p) cudaFreeHost(p);
+        p = q; cap = n;
+    }
 };
 
 struct GpuWorker {
@@ -274,8 +282,8 @@ void addStatsBlock(Stats* s, const std::vector<int64_t>& blk, int64_t C) {
 // writer threads consume (src/writerthread.cpp:37-48).
 // ---------------------------------------------------------------------------------------------------------------
 struct TextChunk {
-    uint8_t* p = nullptr;      // pinned
-    size_t cap = 0, n = 0;
+    Pinned<uint8_t> buf;        // the text: n bytes
+    size_t n = 0;
     bool last = false;
 };
 
@@ -294,20 +302,6 @@ struct ChunkQueue {
         return c;
     }
 };
-
-TextChunk* newChunk(size_t cap) {
-    TextChunk* c = new TextChunk();
-    if (cudaMallocHost((void**)&c->p, cap) != cudaSuccess) error_exit("fastplong_gpu: cudaMallocHost failed");
-    c->cap = cap;
-    return c;
-}
-void growChunk(TextChunk* c, size_t cap) {
-    uint8_t* q = nullptr;
-    if (cudaMallocHost((void**)&q, cap) != cudaSuccess) error_exit("fastplong_gpu: cudaMallocHost failed");
-    memcpy(q, c->p, c->n);
-    cudaFreeHost(c->p);
-    c->p = q; c->cap = cap;
-}
 
 // Largest prefix of buf[0..n) that ends at a record boundary: a newline followed by an '@' line whose line-after-next
 // starts with '+' (a quality line may start with '@', but then the line two below it is a sequence, not a '+' line).
@@ -665,7 +659,11 @@ bool SingleEndProcessor::process() {
         const size_t kChunk = getenv("FPL_CHUNK_KB") ? (size_t)std::max(1L, atol(getenv("FPL_CHUNK_KB"))) << 10 : (size_t)32 << 20;
         std::vector<ChunkQueue> queues(T);
         ChunkQueue freeList;
-        for (int i = 0; i < T + 2; i++) freeList.push(newChunk(kChunk + (8u << 20)));
+        for (int i = 0; i < T + 2; i++) {
+            TextChunk* c = new TextChunk();
+            c->buf.resize(kChunk + (8u << 20));
+            freeList.push(c);
+        }
         FILE* fp = fopen(mOptions->in.c_str(), "rb");
         if (!fp) error_exit("Failed to open file: " + mOptions->in);
         WriterThread* left = mLeftWriter;
@@ -683,18 +681,18 @@ bool SingleEndProcessor::process() {
             long k = 0;
             bool eof = false;
             while (!eof && !notStrict) {
-                if (cur->cap - cur->n < kChunk) growChunk(cur, cur->cap * 2);
-                const size_t got = fread(cur->p + cur->n, 1, kChunk, fp);
+                if (cur->buf.cap - cur->n < kChunk) cur->buf.resize(cur->buf.cap * 2, cur->n);
+                const size_t got = fread(cur->buf.p + cur->n, 1, kChunk, fp);
                 cur->n += got;
                 eof = got < kChunk;
-                size_t cut = eof ? cur->n : recordBoundary(cur->p, cur->n);
+                size_t cut = eof ? cur->n : recordBoundary(cur->buf.p, cur->n);
                 if (!eof && cut == 0) continue;                       // one record larger than the chunk: keep reading
                 TextChunk* next = nullptr;
                 if (!eof) {
                     next = freeList.pop();
-                    if (next->cap < cur->n - cut + kChunk) growChunk(next, cur->n - cut + kChunk + (8u << 20));
                     next->n = cur->n - cut;
-                    memcpy(next->p, cur->p + cut, next->n);
+                    if (next->buf.cap < next->n + kChunk) next->buf.resize(next->n + kChunk + (8u << 20));
+                    memcpy(next->buf.p, cur->buf.p + cut, next->n);
                 }
                 cur->n = cut; cur->last = eof;
                 queues[k % T].push(cur);
@@ -736,17 +734,17 @@ bool SingleEndProcessor::process() {
                 while (failedW && k - written(failedW) > backlog && !notStrict) usleep(200);
                 // four newlines per record: count them to size the record tables
                 size_t nl = 0;
-                for (const uint8_t* q = c->p, *e = c->p + c->n; (q = (const uint8_t*)memchr(q, '\n', (size_t)(e - q))) != nullptr; q++) nl++;
+                for (const uint8_t* q = c->buf.p, *e = c->buf.p + c->n; (q = (const uint8_t*)memchr(q, '\n', (size_t)(e - q))) != nullptr; q++) nl++;
                 const size_t cap = nl / 4 + 16;
                 if (recs.size() < cap) { recs.resize(cap); res.resize(cap); }
                 int64_t n = 0, used = 0;
-                const int rc = fpl_process_fastq_host(w.ctx, c->p, (int64_t)c->n, c->last ? 1 : 0, recs.data(), res.data(),
+                const int rc = fpl_process_fastq_host(w.ctx, c->buf.p, (int64_t)c->n, c->last ? 1 : 0, recs.data(), res.data(),
                                                       (int64_t)cap, &n, &used);
                 if (rc < 0) check(rc, "fpl_process_fastq_host");
                 if (rc == 1 || (size_t)used != c->n) { notStrict = 1; skipChunk(); continue; }
                 string* outstr = new string();
                 string* failedOut = new string();
-                const char* text = (const char*)c->p;
+                const char* text = (const char*)c->buf.p;
                 // FPL_DEVICE_EMIT=1: the two output strings are assembled on the device from the chunk it still holds
                 // (fpl_emit_fastq_host: first call builds and reports the sizes, second call copies); the loop below then
                 // only applies the per-read side effects
@@ -789,7 +787,6 @@ bool SingleEndProcessor::process() {
             if (freeList.q.empty()) break;
             TextChunk* c = freeList.q.front(); freeList.q.pop_front();
             l.unlock();
-            cudaFreeHost(c->p);
             delete c;
         }
         if (notStrict) {

@@ -5,6 +5,7 @@
 #include "fake/cuda.h"
 #include "fake/nvrtc.h"
 #include <dlfcn.h>
+#include <map>
 #include <mutex>
 #include <string>
 
@@ -45,6 +46,51 @@ extern "C" long long emu_live_allocs() { return emu::live_allocs; }
 // -> the count it replaces: > 0 when the allocation it was set for never came
 extern "C" long long emu_fail_alloc(long long k) { const long long was = emu::fail_alloc_in; emu::fail_alloc_in = k; return was; }
 extern "C" long long emu_blocks() { return (long long)emu::block_serial; }
+
+// ---------------- streams and events (fake/cuda_runtime.h): ids never reused; the live ones, an event with its timestamp ----------------
+namespace emu {
+namespace {
+std::mutex handle_mu;                   // host threads with a context each create and destroy their own
+std::map<const void*, double> handles;
+uintptr_t last_handle = 0x100000;
+long long fail_handle_in = 0, bad_handles = 0, failed_kind = 0;
+}  // namespace
+void* handle_new(int kind) {
+    std::lock_guard<std::mutex> lock(handle_mu);
+    if (fail_handle_in > 0 && --fail_handle_in == 0) { failed_kind = kind; return nullptr; }
+    last_handle += 16;
+    handles[(const void*)last_handle] = 0;
+    return (void*)last_handle;
+}
+double* handle(const void* h) {
+    std::lock_guard<std::mutex> lock(handle_mu);
+    auto it = handles.find(h);
+    if (it == handles.end()) { bad_handles++; return nullptr; }
+    return &it->second;
+}
+bool handle_free(const void* h) {
+    std::lock_guard<std::mutex> lock(handle_mu);
+    if (handles.erase(h)) return true;
+    bad_handles++;
+    return false;
+}
+}  // namespace emu
+extern "C" long long emu_live_handles() { std::lock_guard<std::mutex> lock(emu::handle_mu); return (long long)emu::handles.size(); }
+extern "C" long long emu_bad_handles() { std::lock_guard<std::mutex> lock(emu::handle_mu); return emu::bad_handles; }
+// -> the count it replaces: > 0 when the creation it was set for never came
+extern "C" long long emu_fail_handle(long long k) {
+    std::lock_guard<std::mutex> lock(emu::handle_mu);
+    const long long was = emu::fail_handle_in;
+    emu::fail_handle_in = k;
+    return was;
+}
+// -> what the creation that emu_fail_handle made fail created (EMU_STREAM, EMU_EVENT, EMU_TIMING_EVENT; 0: none), and forgets it
+extern "C" long long emu_failed_handle_kind() {
+    std::lock_guard<std::mutex> lock(emu::handle_mu);
+    const long long k = emu::failed_kind;
+    emu::failed_kind = 0;
+    return k;
+}
 
 // ---------------- NVRTC + driver: kernels "compiled" for the host ----------------
 struct EmuNvrtcProgram { std::string src, log, so; };

@@ -4,10 +4,11 @@
 #include "../emu_cuda.h"
 #include <time.h>
 
-enum cudaError_t { cudaSuccess = 0, cudaErrorInvalidValue = 1, cudaErrorMemoryAllocation = 2, cudaErrorNotReady = 600 };
+enum cudaError_t { cudaSuccess = 0, cudaErrorInvalidValue = 1, cudaErrorMemoryAllocation = 2, cudaErrorInvalidResourceHandle = 400,
+                   cudaErrorNotReady = 600 };
 enum cudaMemcpyKind { cudaMemcpyHostToHost = 0, cudaMemcpyHostToDevice = 1, cudaMemcpyDeviceToHost = 2, cudaMemcpyDeviceToDevice = 3, cudaMemcpyDefault = 4 };
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2, cudaFuncAttributeMaxDynamicSharedMemorySize = 8 };
-struct EmuEvent { double t; };
+struct EmuEvent;
 typedef EmuEvent* cudaEvent_t;
 static inline const char* cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : "emulated runtime error"; }
 static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
@@ -30,28 +31,72 @@ template <class T> static inline cudaError_t cudaMalloc(T** p, size_t n) { *p = 
 template <class T> static inline cudaError_t cudaMallocHost(T** p, size_t n) { *p = (T*)emu_alloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
 static inline cudaError_t cudaFree(void* p) { if (p) { emu::live_allocs--; free(p); } return cudaSuccess; }
 static inline cudaError_t cudaFreeHost(void* p) { if (p) { emu::live_allocs--; free(p); } return cudaSuccess; }
+// Streams and events are ids that are never reused, kept by emu_core.cpp (an event with its timestamp): emu_live_handles counts the
+// live ones; emu::fail_handle_in = k > 0 makes the k-th creation from now fail, once, and write EMU_POISON as the handle
+// (emu_fail_handle); a call that gets a handle that is not live (poison, destroyed) fails and counts in emu_bad_handles.  The null
+// stream is the default stream.
+enum { EMU_STREAM = 1, EMU_EVENT = 2, EMU_TIMING_EVENT = 3 };
+#define EMU_POISON ((void*)0xBADBAD0)
+namespace emu {
+void* handle_new(int kind);             // nullptr: this creation fails
+double* handle(const void* h);          // the live handle's timestamp; nullptr (and counted) when h is not live
+bool handle_free(const void* h);
+}  // namespace emu
+template <class H> static inline cudaError_t emu_create(H* h, int kind) {
+    void* p = emu::handle_new(kind);
+    *h = (H)(p ? p : EMU_POISON);
+    return p ? cudaSuccess : cudaErrorMemoryAllocation;
+}
+static inline bool emu_stream_ok(cudaStream_t s) { return !s || emu::handle(s); }
+#define EMU_CHECK_STREAM(s) do { if (!emu_stream_ok(s)) return cudaErrorInvalidResourceHandle; } while (0)
 static inline cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { if (n) memmove(d, s, n); return cudaSuccess; }
-static inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t = nullptr) { if (n) memmove(d, s, n); return cudaSuccess; }
+static inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t st = nullptr) {
+    EMU_CHECK_STREAM(st);
+    if (n) memmove(d, s, n);
+    return cudaSuccess;
+}
 static inline cudaError_t cudaMemcpy2DAsync(void* d, size_t dpitch, const void* s, size_t spitch, size_t width, size_t height, cudaMemcpyKind,
-                                            cudaStream_t = nullptr) {
+                                            cudaStream_t st = nullptr) {
+    EMU_CHECK_STREAM(st);
     for (size_t r = 0; r < height; r++) memmove((char*)d + r * dpitch, (const char*)s + r * spitch, width);
     return cudaSuccess;
 }
 static inline cudaError_t cudaMemset(void* d, int v, size_t n) { if (n) memset(d, v, n); return cudaSuccess; }
-static inline cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t = nullptr) { if (n) memset(d, v, n); return cudaSuccess; }
-static inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { *s = malloc(8); return cudaSuccess; }
-static inline cudaError_t cudaStreamCreate(cudaStream_t* s) { *s = malloc(8); return cudaSuccess; }
-static inline cudaError_t cudaStreamDestroy(cudaStream_t s) { free(s); return cudaSuccess; }
-static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
+static inline cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t st = nullptr) {
+    EMU_CHECK_STREAM(st);
+    if (n) memset(d, v, n);
+    return cudaSuccess;
+}
+static inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { return emu_create(s, EMU_STREAM); }
+static inline cudaError_t cudaStreamCreate(cudaStream_t* s) { return emu_create(s, EMU_STREAM); }
+static inline cudaError_t cudaStreamDestroy(cudaStream_t s) { return s && emu::handle_free(s) ? cudaSuccess : cudaErrorInvalidResourceHandle; }
+static inline cudaError_t cudaStreamSynchronize(cudaStream_t s) { EMU_CHECK_STREAM(s); return cudaSuccess; }
 static inline double emu_now_ms() { timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return ts.tv_sec * 1e3 + ts.tv_nsec * 1e-6; }
-static inline cudaError_t cudaEventCreate(cudaEvent_t* e) { *e = new EmuEvent{0}; return cudaSuccess; }
-static inline cudaError_t cudaEventCreateWithFlags(cudaEvent_t* e, unsigned) { *e = new EmuEvent{0}; return cudaSuccess; }
-static inline cudaError_t cudaEventDestroy(cudaEvent_t e) { delete e; return cudaSuccess; }
-static inline cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t = nullptr) { e->t = emu_now_ms(); return cudaSuccess; }
-static inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }
-static inline cudaError_t cudaEventQuery(cudaEvent_t) { return cudaSuccess; }
-static inline cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t a, cudaEvent_t b) { *ms = (float)(b->t - a->t); return cudaSuccess; }
-static inline cudaError_t cudaStreamWaitEvent(cudaStream_t, cudaEvent_t, unsigned = 0) { return cudaSuccess; }
+static inline cudaError_t cudaEventCreate(cudaEvent_t* e) { return emu_create(e, EMU_TIMING_EVENT); }
+static inline cudaError_t cudaEventCreateWithFlags(cudaEvent_t* e, unsigned flags) {
+    return emu_create(e, flags & cudaEventDisableTiming ? EMU_EVENT : EMU_TIMING_EVENT);
+}
+static inline cudaError_t cudaEventDestroy(cudaEvent_t e) { return emu::handle_free(e) ? cudaSuccess : cudaErrorInvalidResourceHandle; }
+static inline cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t s = nullptr) {
+    double* t = emu::handle(e);
+    EMU_CHECK_STREAM(s);
+    if (!t) return cudaErrorInvalidResourceHandle;
+    *t = emu_now_ms();
+    return cudaSuccess;
+}
+static inline cudaError_t cudaEventSynchronize(cudaEvent_t e) { return emu::handle(e) ? cudaSuccess : cudaErrorInvalidResourceHandle; }
+static inline cudaError_t cudaEventQuery(cudaEvent_t e) { return emu::handle(e) ? cudaSuccess : cudaErrorInvalidResourceHandle; }
+static inline cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t a, cudaEvent_t b) {
+    const double *ta = emu::handle(a), *tb = emu::handle(b);
+    if (!ta || !tb) return cudaErrorInvalidResourceHandle;
+    *ms = (float)(*tb - *ta);
+    return cudaSuccess;
+}
+static inline cudaError_t cudaStreamWaitEvent(cudaStream_t s, cudaEvent_t e, unsigned = 0) {
+    const bool ok = emu::handle(e) != nullptr;
+    EMU_CHECK_STREAM(s);
+    return ok ? cudaSuccess : cudaErrorInvalidResourceHandle;
+}
 template <class F> static inline cudaError_t cudaFuncSetAttribute(F, int, int) { return cudaSuccess; }
 
 // ---- host forms of the PTX wrappers (their definitions are cut out of fpl_device.cuh / fpl_stats.cu) ----

@@ -187,13 +187,20 @@ def build_binary():
 def emulated_library():
     """ctypes handle of the emulated library (emulator switches: emu_set_cp_async_lazy, emu_collectives, emu_blocks; emu_live_allocs:
     cudaMalloc / cudaMallocHost blocks not yet freed; emu_fail_alloc(k): the k-th allocation from now fails, once, 0 = none; it
-    returns the count it replaces, > 0 when that allocation never came)"""
+    returns the count it replaces, > 0 when that allocation never came.  emu_live_handles, emu_fail_handle(k): the same for stream
+    and event creations, where a failed one writes a poison handle; emu_failed_handle_kind(): what that creation was (EMU_STREAM,
+    EMU_EVENT, EMU_TIMING_EVENT, 0: none), then 0; emu_bad_handles: calls that got a handle that was not live)"""
     lib = C.CDLL(build_library())
     lib.emu_set_cp_async_lazy.argtypes = [C.c_int]
     lib.emu_collectives.restype = lib.emu_blocks.restype = lib.emu_live_allocs.restype = C.c_longlong
-    lib.emu_fail_alloc.argtypes = [C.c_longlong]
-    lib.emu_fail_alloc.restype = C.c_longlong
+    lib.emu_live_handles.restype = lib.emu_bad_handles.restype = lib.emu_failed_handle_kind.restype = C.c_longlong
+    for f in (lib.emu_fail_alloc, lib.emu_fail_handle):
+        f.argtypes = [C.c_longlong]
+        f.restype = C.c_longlong
     return lib
+
+
+EMU_STREAM, EMU_EVENT, EMU_TIMING_EVENT = 1, 2, 3       # emu_failed_handle_kind (tests/simt/fake/cuda_runtime.h)
 
 
 class _Bound:

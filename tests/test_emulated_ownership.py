@@ -1,13 +1,17 @@
-"""Who owns the library's device memory, on the emulated library (tests/simt_emu.py), whose cudaMalloc / cudaMallocHost count the
-blocks alive (emu_live_allocs) and fail the k-th allocation from now on request (emu_fail_alloc).  A context frees everything its
-entry points allocated when it is destroyed; an allocation that fails anywhere in a call makes the call fail and leaks nothing;
-fpl_stats_reserve is all or nothing; a report or emit build that failed gives the same bytes when it is called again."""
+"""Who owns the library's device memory, streams and events, on the emulated library (tests/simt_emu.py), whose cudaMalloc /
+cudaMallocHost count the blocks alive (emu_live_allocs) and fail the k-th allocation from now on request (emu_fail_alloc), and whose
+stream and event creations do the same (emu_live_handles, emu_fail_handle) and count the calls that get a handle that is not live
+(emu_bad_handles).  A context frees everything its entry points allocated or created when it is destroyed; an allocation that fails
+anywhere in a call makes the call fail and leaks nothing; so does a stream or event creation, except a timing event, whose launch
+then runs untimed; fpl_stats_reserve is all or nothing; a report or emit build that failed gives the same bytes when it is called
+again."""
 import gc
 
 import numpy as np
 import pytest
 
 import cases
+import layouts
 import simt_emu
 from fastplong_b200 import abi, synth
 from fastplong_b200.binding import FplError
@@ -173,3 +177,98 @@ def test_a_failed_fpl_stats_reserve_changes_nothing(lib):
     np.testing.assert_array_equal(e.counters(), fresh.counters())
     e.close()
     fresh.close()
+
+
+# ENTRIES, fpl_reset, and fpl_process_host on three reads whose slots lie 1 MiB apart: at FPL_PIECE_MB=1 it uploads them on its
+# copy stream in three pieces, an event each
+PIECES = layouts.relayout(BATCH.slice(0, 3), align=1 << 20)
+HANDLE_ENTRIES = {**ENTRIES, "fpl_process_host in pieces": (None, lambda e: e.process(PIECES), False),
+                  "fpl_reset": (lambda e: e.process(BATCH), lambda e: e.reset(), False)}
+
+
+def held(lib):
+    """live blocks, live streams and events, calls that got a handle that was not live"""
+    return live(lib), lib.emu_live_handles(), lib.emu_bad_handles()
+
+
+@pytest.mark.parametrize("timing", [False, True], ids=["untimed", "timed"])
+@pytest.mark.parametrize("opt", [PLAIN, EXT], ids=["plain", "mask_break"])
+def test_every_entry_point_releases_its_streams_events_and_blocks(lib, monkeypatch, opt, timing):
+    monkeypatch.setenv("FPL_PIECE_MB", "1")
+    base = held(lib)
+    for entry, (before, call, _) in HANDLE_ENTRIES.items():
+        e = engine(opt)
+        e.set_timing(timing)
+        if before:
+            before(e)
+        call(e)
+        close(e)
+        assert held(lib) == base, entry
+
+
+def test_a_failed_stream_creation_in_fpl_create_leaks_nothing(lib):
+    base, k = held(lib), 0
+    while True:
+        k += 1
+        lib.emu_fail_handle(k)
+        try:
+            engine(PLAIN).close()
+            failed = False
+        except FplError:
+            failed = True
+        pending, kind = lib.emu_fail_handle(0), lib.emu_failed_handle_kind()
+        assert held(lib) == base, f"creation {k} failed: leak or dead handle"
+        if pending:
+            assert not failed and k > 1
+            return
+        assert failed and kind == simt_emu.EMU_STREAM, f"creation {k} failed, fpl_create succeeded"
+
+
+@pytest.mark.parametrize("timing", [False, True], ids=["untimed", "timed"])
+@pytest.mark.parametrize("entry", list(HANDLE_ENTRIES))
+@pytest.mark.parametrize("opt", [PLAIN, EXT], ids=["plain", "mask_break"])
+def test_a_failed_stream_or_event_creation_leaks_nothing(lib, monkeypatch, opt, entry, timing):
+    """every stream or event the call creates fails once in turn: the call fails, except where a timing event failed, whose launch
+    then runs untimed and is counted; nothing leaks, no call gets a poisoned or released handle, and the context's next batch gives
+    the records, Stats and counters of a context that never failed"""
+    monkeypatch.setenv("FPL_PIECE_MB", "1")
+    before, call, _ = HANDLE_ENTRIES[entry]
+
+    def run(k, skip=False):
+        """-> (the call failed, what the k-th creation made (0: it never came), timed launches, launches, the next batch's
+        records, Stats and counters); skip: the call is left out"""
+        e = engine(opt)
+        e.set_timing(timing)
+        if before:
+            before(e)
+        lib.emu_fail_handle(k)
+        failed = False
+        try:
+            if not skip:
+                call(e)
+        except FplError:
+            failed = True
+        kind = lib.emu_failed_handle_kind() if lib.emu_fail_handle(0) == 0 else 0
+        timed = sum(n for _, n in e.kernel_times().values())
+        launches = e.launch_count
+        res = e.process(BATCH)
+        after = [res.tobytes(), *(e.stats(w).tobytes() for w in (0, 1)), e.counters().tobytes()]
+        close(e)
+        return failed, kind, timed, launches, after
+
+    _, _, timed, launches, after = run(0)
+    after_skip = run(0, skip=True)[4]
+    base, k = held(lib), 0
+    while True:
+        k += 1
+        failed, kind, got_timed, got_launches, got_after = run(k)
+        assert held(lib) == base, f"{entry}: creation {k} failed: leak or dead handle"
+        if not kind:
+            return
+        if kind == simt_emu.EMU_TIMING_EVENT:
+            assert not failed, f"{entry}: timing event {k} failed, so did the call"
+            assert (got_timed, got_launches) == (timed - 1, launches), f"{entry}: timing event {k} failed: timed launches, launches"
+            assert got_after == after, f"{entry}: the batch after timing event {k} failed"
+        else:
+            assert failed, f"{entry}: creation {k} failed, the call succeeded"
+            assert got_after == after_skip, f"{entry}: the batch after creation {k} failed"
