@@ -2,7 +2,7 @@
 import ctypes as C
 import numpy as np
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 COMM_ID_BYTES = 128        # FPL_COMM_ID_BYTES == sizeof(ncclUniqueId)
 MAX_ADAPTER_LEN = 1024
 MAX_ADAPTERS = 1024

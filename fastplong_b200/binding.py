@@ -60,6 +60,8 @@ def load_library():
     lib.fpl_comm_agree_cycles.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     lib.fpl_allreduce_stats.argtypes = [C.c_void_p, C.c_int64]
     lib.fpl_merge_stats.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int]
+    lib.fpl_state_export.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
+    lib.fpl_state_merge.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int]
     lib.fpl_eval_adapter_kmers.argtypes = [C.c_int, C.POINTER(FplBatch), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                            C.POINTER(C.c_int64)]
     lib.fpl_eval_pick_adapter.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_char_p, C.c_int32]
@@ -83,7 +85,7 @@ EXPORTS = ["fpl_last_error", "fpl_abi_version", "fpl_create", "fpl_destroy", "fp
            "fpl_sync", "fpl_stream", "fpl_last_segments", "fpl_last_mask_regions", "fpl_fetch_results", "fpl_stats_cycles", "fpl_stats_reserve", "fpl_stats_download",
            "fpl_stats_device_ptr", "fpl_counter_words", "fpl_counters_download", "fpl_counters_device_ptr",
            "fpl_comm_unique_id", "fpl_comm_init", "fpl_comm_destroy", "fpl_comm_size", "fpl_comm_agree_cycles", "fpl_allreduce_stats",
-           "fpl_merge_stats",
+           "fpl_merge_stats", "fpl_state_export", "fpl_state_merge",
            "fpl_eval_adapter_kmers", "fpl_eval_pick_adapter", "fpl_report_json", "fpl_keep_read_lists", "fpl_report_html", "fpl_reset", "fpl_last_kernel_times", "fpl_launch_count", "fpl_set_timing"]
 
 
@@ -322,6 +324,33 @@ class Engine:
         The others are not modified and may be used again at once.  Same device, options and adapters, or FplError."""
         arr = (C.c_void_p * max(1, len(others)))(*(o.h.value if o.h else None for o in others))
         self._check(self.lib.fpl_merge_stats(self.h, arr, len(others)))
+
+    def export_state(self):
+        """The engine's accumulated state as a self-contained byte image (fpl_state_export; layout in include/fplgpu.h): both
+        Stats blocks, the counters, the read lists and their flags, under the engine's options and adapters.  The engine is not
+        changed."""
+        n = C.c_int64()
+        rc = self.lib.fpl_state_export(self.h, None, 0, C.byref(n))
+        if rc < 0:
+            self._check(rc)
+        buf = np.empty(n.value, dtype=np.uint8)
+        self._check(self.lib.fpl_state_export(self.h, buf.ctypes.data, buf.size, C.byref(n)))
+        return buf.tobytes()
+
+    def merge_state(self, *images):
+        """Merge images of export_state() (bytes, bytearray or uint8 numpy arrays), in that order, into this engine
+        (fpl_state_merge): the engine ends as merge() of the engines that exported them would leave it, whichever device or
+        process they ran in.  Same options (the device aside) and adapters, a valid image, or FplError with the engine
+        unchanged."""
+        arrs = []
+        for im in images:
+            a = im if isinstance(im, np.ndarray) else np.frombuffer(im, dtype=np.uint8)
+            if a.dtype != np.uint8 or a.ndim != 1:
+                raise FplError("merge_state: an image is bytes, a bytearray or a 1-D uint8 array")
+            arrs.append(np.ascontiguousarray(a))
+        ptrs = (C.c_void_p * max(1, len(arrs)))(*(a.ctypes.data for a in arrs))
+        sizes = (C.c_int64 * max(1, len(arrs)))(*(a.size for a in arrs))
+        self._check(self.lib.fpl_state_merge(self.h, ptrs, sizes, len(arrs)))
 
     # --- multi-GPU merge (one process per GPU): Stats::merge / FilterResult::merge as NCCL all-reduces ---
     @staticmethod

@@ -224,6 +224,8 @@ struct fpl_ctx {
     // fpl_merge_stats: the sources' table (k_merge_stats) and the event that orders the streams
     DevBuf<MergeSrc> d_merge;
     Event merge_ev;
+    DevBuf<unsigned long long> d_state_stage;   // fpl_state_merge: the images' Stats and counter sections
+
     // timing (Timed): the recorded start / end pairs not yet collected, and the collected events for reuse
     struct Ev { int k; Event a, b; };
     std::vector<Ev> events;
@@ -2049,5 +2051,201 @@ extern "C" int fpl_merge_stats(fpl_ctx* c, fpl_ctx* const* src, int n_src) {
     L.complete = complete; L.merged = merged;
     c->rep.built = false; c->html.built = false;
     CK(cudaGetLastError());
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// fpl_state_export / fpl_state_merge: a context's state as a byte image (layout: include/fplgpu.h) and images merged with
+// fpl_merge_stats' semantics (Stats::merge, src/stats.cpp:1013-1082; FilterResult::merge, src/filterresult.cpp:28-61).  The
+// images' Stats and counter sections are staged in one device buffer, where each image's compact blocks (capacity = rows) are a
+// k_merge_stats source as they are; the read-list entries are copied behind dst's.
+// ------------------------------------------------------------------------------------------------------------------
+#if defined(__BYTE_ORDER__) && __BYTE_ORDER__ != __ORDER_LITTLE_ENDIAN__
+#error "state images are little-endian: the library supports little-endian hosts only"
+#endif
+
+namespace {
+
+enum { SI_MAGIC, SI_FORMAT, SI_ABI, SI_TOTAL, SI_N_ADAPTERS, SI_ADAPTER_BYTES, SI_COUNTER_WORDS, SI_ROWS, SI_USED, SI_REDUCED,
+       SI_KEEP, SI_COMPLETE, SI_MERGED, SI_LIST0, SI_LIST1, SI_WORDS };
+// the fpl_options bytes in the image: what fpl_merge_stats compares (device up to reserved) but device
+const size_t kOptBegin = offsetof(fpl_options, trim_front), kOptEnd = offsetof(fpl_options, reserved);
+const int64_t kOptAt = 8 * SI_WORDS;
+static_assert(offsetof(fpl_options, device) + sizeof(int32_t) == offsetof(fpl_options, trim_front), "device precedes trim_front");
+static_assert(kOptAt + (int64_t)(kOptEnd - kOptBegin) + 4 == FPL_STATE_HEADER_BYTES, "FPL_STATE_HEADER_BYTES");
+static_assert(sizeof(HtmlEntry) == 8, "list entries are 8 bytes in the image");
+
+int64_t pad8(int64_t n) { return (n + 7) & ~(int64_t)7; }
+
+int64_t adapter_section_bytes(const std::vector<std::string>& a) {
+    int64_t n = 0;
+    for (const std::string& s : a) n += 8 + pad8((int64_t)s.size());
+    return n;
+}
+
+// one validated image: its flags, list lengths and where its sections are
+struct StateImage {
+    int64_t rows, used, reduced, n[2];
+    bool complete, merged;
+    const uint8_t* stats;                   // pre and post Stats, then the counters: contiguous
+    const uint8_t* list[2];
+};
+
+// Validation of image i against dst, on the host, reading nothing outside [p, p + n)
+int parse_image(const fpl_ctx* c, int i, const uint8_t* p, int64_t n, StateImage& im) {
+    if (!p) return fail("fpl_state_merge: image %d is null", i);
+    if (n < 0) return fail("fpl_state_merge: image %d has a negative size (%lld)", i, (long long)n);
+    if (n < FPL_STATE_HEADER_BYTES)
+        return fail("fpl_state_merge: image %d is truncated: %lld bytes, the header alone is %d", i, (long long)n, FPL_STATE_HEADER_BYTES);
+    int64_t h[SI_WORDS];
+    memcpy(h, p, sizeof(h));
+    if ((uint64_t)h[SI_MAGIC] != FPL_STATE_MAGIC) return fail("fpl_state_merge: image %d is not a state image (bad magic number)", i);
+    if (h[SI_FORMAT] != FPL_STATE_FORMAT)
+        return fail("fpl_state_merge: image %d has image format %lld, this library reads format %d", i, (long long)h[SI_FORMAT],
+                    FPL_STATE_FORMAT);
+    if (h[SI_ABI] != FPL_ABI_VERSION)
+        return fail("fpl_state_merge: image %d was written with FPL_ABI_VERSION %lld, this library is %d", i, (long long)h[SI_ABI],
+                    FPL_ABI_VERSION);
+    if (h[SI_TOTAL] != n)
+        return fail("fpl_state_merge: image %d: its header says %lld bytes, %lld were given (truncated, or trailing bytes)", i,
+                    (long long)h[SI_TOTAL], (long long)n);
+    for (int k = SI_N_ADAPTERS; k < SI_WORDS; k++)
+        if (h[k] < 0) return fail("fpl_state_merge: image %d: header word %d is negative (%lld)", i, k, (long long)h[k]);
+    for (int k = SI_KEEP; k <= SI_MERGED; k++)
+        if (h[k] > 1) return fail("fpl_state_merge: image %d: header word %d is a flag, not %lld", i, k, (long long)h[k]);
+    const int64_t A = h[SI_ADAPTER_BYTES], cw = h[SI_COUNTER_WORDS], rows = h[SI_ROWS], n0 = h[SI_LIST0], n1 = h[SI_LIST1];
+    if (rows != std::max(h[SI_USED], h[SI_REDUCED]))
+        return fail("fpl_state_merge: image %d: rows %lld != max(used_cycles, reduced_rows)", i, (long long)rows);
+    // each length within the image before any product of them: the sum below cannot overflow
+    if (A > n || cw > n / 8 || rows > n / 256 || n0 > n / 8 || n1 > n / 8 ||
+        FPL_STATE_HEADER_BYTES + A + 8 * (2 * FPL_STATS_WORDS(rows) + cw + n0 + n1) != n)
+        return fail("fpl_state_merge: image %d: the section lengths do not add up to its %lld bytes", i, (long long)n);
+    if (memcmp(p + kOptAt, reinterpret_cast<const char*>(&c->P.opt) + kOptBegin, kOptEnd - kOptBegin))
+        return fail("fpl_state_merge: image %d was created with other options than the destination", i);
+    // A == dst's adapter section and the sum above hold: walking dst's lengths stays inside the section
+    if (h[SI_N_ADAPTERS] != (int64_t)c->adapter_str.size() || A != adapter_section_bytes(c->adapter_str))
+        return fail("fpl_state_merge: image %d was created with another adapter list than the destination", i);
+    const uint8_t* q = p + FPL_STATE_HEADER_BYTES;
+    for (const std::string& s : c->adapter_str) {
+        int64_t len;
+        memcpy(&len, q, 8);
+        if (len != (int64_t)s.size() || memcmp(q + 8, s.data(), s.size()))
+            return fail("fpl_state_merge: image %d was created with another adapter list than the destination", i);
+        q += 8 + pad8(len);
+    }
+    if (cw != c->counter_words)
+        return fail("fpl_state_merge: image %d has %lld counter words, the destination %lld", i, (long long)cw,
+                    (long long)c->counter_words);
+    im.rows = rows; im.used = h[SI_USED]; im.reduced = h[SI_REDUCED];
+    im.n[0] = n0; im.n[1] = n1;
+    im.complete = h[SI_COMPLETE] != 0; im.merged = h[SI_MERGED] != 0;
+    im.stats = q;
+    im.list[0] = q + 8 * (2 * FPL_STATS_WORDS(rows) + cw);
+    im.list[1] = im.list[0] + 8 * n0;
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int fpl_state_export(fpl_ctx* c, uint8_t* out, int64_t cap, int64_t* n_bytes) {
+    g_err[0] = 0;
+    if (!c || !n_bytes) return fail("fpl_state_export: null argument");
+    const FplLists& L = c->lists;
+    const int64_t rows = std::max(c->used_cycles, c->reduced_rows), sw = FPL_STATS_WORDS(rows), cw = c->counter_words;
+    const int64_t A = adapter_section_bytes(c->adapter_str);
+    const int64_t total = FPL_STATE_HEADER_BYTES + A + 8 * (2 * sw + cw + L.n[0] + L.n[1]);
+    *n_bytes = total;
+    if (!out || cap < total) return 1;
+    CK(cudaSetDevice(c->device));
+    memset(out, 0, (size_t)(FPL_STATE_HEADER_BYTES + A));
+    const int64_t h[SI_WORDS] = {(int64_t)FPL_STATE_MAGIC, FPL_STATE_FORMAT, FPL_ABI_VERSION, total, (int64_t)c->adapter_str.size(), A, cw,
+                                 rows, c->used_cycles, c->reduced_rows, L.keep, L.complete, L.merged, L.n[0], L.n[1]};
+    memcpy(out, h, sizeof(h));
+    memcpy(out + kOptAt, reinterpret_cast<const char*>(&c->P.opt) + kOptBegin, kOptEnd - kOptBegin);
+    uint8_t* q = out + FPL_STATE_HEADER_BYTES;
+    for (const std::string& s : c->adapter_str) {
+        const int64_t len = (int64_t)s.size();
+        memcpy(q, &len, 8);
+        memcpy(q + 8, s.data(), s.size());
+        q += 8 + pad8(len);
+    }
+    const size_t W = sizeof(unsigned long long);
+    for (int w = 0; w < 2; w++) {
+        uint8_t* blk = q + W * sw * w;
+        if (rows)       // rows b*C + c of the block go to b*rows + c
+            CK(cudaMemcpy2DAsync(blk, W * rows, c->d_stats[w], W * c->C, W * rows, 16, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(blk + W * 16 * rows, c->d_stats[w] + 16 * c->C, W * FPL_STATS_TAIL, cudaMemcpyDeviceToHost, c->stream));
+    }
+    q += W * 2 * sw;
+    CK(cudaMemcpyAsync(q, c->d_counters, W * cw, cudaMemcpyDeviceToHost, c->stream));
+    q += W * cw;
+    for (int w = 0; w < 2; w++) {
+        if (L.n[w]) CK(cudaMemcpyAsync(q, L.d[w], sizeof(HtmlEntry) * L.n[w], cudaMemcpyDeviceToHost, c->stream));
+        q += sizeof(HtmlEntry) * L.n[w];
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    collect_times(c);
+    return 0;
+}
+
+extern "C" int fpl_state_merge(fpl_ctx* c, const uint8_t* const* images, const int64_t* n_bytes, int n_images) {
+    g_err[0] = 0;
+    if (!c) return fail("fpl_state_merge: null destination context");
+    if (n_images < 0) return fail("fpl_state_merge: negative number of images (%d)", n_images);
+    if (n_images > 0 && (!images || !n_bytes)) return fail("fpl_state_merge: null image or size list");
+    std::vector<StateImage> im((size_t)n_images);
+    for (int k = 0; k < n_images; k++)
+        if (parse_image(c, k, images[k], n_bytes[k], im[k])) return -1;
+    if (n_images == 0) return 0;
+    CK(cudaSetDevice(c->device));
+    FplLists& L = c->lists;
+    const int64_t cw = c->counter_words;
+    int64_t rows = 0, used = c->used_cycles, reduced = c->reduced_rows, total[2] = {L.n[0], L.n[1]}, words = 0;
+    bool complete = L.complete, merged = L.merged;
+    for (const StateImage& s : im) {
+        rows = std::max(rows, s.rows);
+        used = std::max(used, s.used);
+        reduced = std::max(reduced, s.reduced);
+        complete = complete && s.complete;
+        merged = merged || s.merged;
+        for (int w = 0; w < 2; w++) total[w] += s.n[w];
+        words += 2 * FPL_STATS_WORDS(s.rows) + cw;
+    }
+    // the capacities first, as fpl_merge_stats grows them
+    if (reserve_cycles(c, rows)) return -1;
+    if (L.keep && (grow_list(c, 0, total[0]) || grow_list(c, 1, total[1]))) return -1;
+    CK(c->d_state_stage.grow(words));
+    CK(c->d_merge.grow(n_images));
+    std::vector<MergeSrc> tab((size_t)n_images);
+    int64_t at = 0;
+    for (int k = 0; k < n_images; k++) {
+        const int64_t sw = FPL_STATS_WORDS(im[k].rows);
+        unsigned long long* d = c->d_state_stage + at;
+        CK(cudaMemcpyAsync(d, im[k].stats, sizeof(unsigned long long) * (2 * sw + cw), cudaMemcpyHostToDevice, c->stream));
+        // the compact blocks as a source of capacity rows: k_merge_stats reads b * rows + c for c < rows, the tail at 16 * rows
+        tab[k] = MergeSrc{{d, d + sw}, d + 2 * sw, im[k].rows, im[k].rows};
+        at += 2 * sw + cw;
+    }
+    CK(cudaMemcpyAsync(c->d_merge, tab.data(), sizeof(MergeSrc) * n_images, cudaMemcpyHostToDevice, c->stream));
+    {
+        Timed t(c, K_MERGE_STATS);
+        launch_merge_stats(c->d_stats[0], c->d_stats[1], c->d_counters, c->C, rows, cw, c->d_merge, n_images, c->stream);
+    }
+    if (L.keep) {
+        for (int w = 0; w < 2; w++)
+            for (const StateImage& s : im) {
+                if (s.n[w])
+                    CK(cudaMemcpyAsync(L.d[w] + L.n[w], s.list[w], sizeof(HtmlEntry) * s.n[w], cudaMemcpyHostToDevice, c->stream));
+                L.n[w] += s.n[w];
+            }
+    } else {
+        complete = false;                     // the images' entries were not taken, as in a call with capture off
+    }
+    c->used_cycles = used; c->reduced_rows = reduced;
+    L.complete = complete; L.merged = merged;
+    c->rep.built = false; c->html.built = false;
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(c->stream));
+    collect_times(c);
     return 0;
 }

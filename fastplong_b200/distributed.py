@@ -4,7 +4,11 @@ src/seprocessor.cpp:108-121).
 
 GPU path: the merge is the C ABI's own (include/fplgpu.h: fpl_comm_init + fpl_allreduce_stats — ncclAllReduce on the
 context's stream); torch.distributed is only the out-of-band channel that carries rank 0's 128-byte rendezvous id and
-gathers the per-read records.  The same shard / gather logic runs on gloo with host blocks in the CPU tests."""
+gathers the per-read records.  The same shard / gather logic runs on gloo with host blocks in the CPU tests.
+
+gather_engine is the other merge: every rank's whole state (fpl_state_export: both Stats blocks, the counters and the per-read
+lists) travels to one rank over the torch.distributed group, which merges the images (fpl_state_merge) and so can write the
+job's HTML report as well as its JSON one."""
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -53,3 +57,35 @@ def gather_records(records, bounds, rank, world_size, group=None):
     out = [None] * world_size
     dist.all_gather_object(out, np.asarray(records), group=group)
     return np.concatenate(out)
+
+
+def gather_engine(engine, root=0, group=None):
+    """Stats::merge / FilterResult::merge of every rank's engine into `root`'s, in rank order, read lists included: each rank
+    exports its state, the images travel to `root` over the torch.distributed group (CUDA uint8 tensors on NCCL, host tensors
+    on any other backend), and `root` merges them (fpl_state_merge).  With contiguous shards (shard()) `root` then holds the
+    whole job: its report_json / report_html are those of one engine over the unsharded input.  The other ranks' engines are
+    not changed.  A refusal (other options or adapters on some rank) raises FplError with `root`'s own state in its engine."""
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    root_global = root if group is None else dist.get_global_rank(group, root)
+    dev = torch.device("cuda", engine.options.device) if dist.get_backend(group) == "nccl" else torch.device("cpu")
+    mine = engine.export_state()
+    sizes = [torch.zeros(1, dtype=torch.int64, device=dev) for _ in range(world)]
+    dist.all_gather(sizes, torch.tensor([len(mine)], dtype=torch.int64, device=dev), group=group)
+    sizes = [int(n.item()) for n in sizes]
+    buf = torch.zeros(max(sizes), dtype=torch.uint8, device=dev)      # gather takes equal shapes: the image, then zeros
+    buf[:len(mine)] = torch.frombuffer(bytearray(mine), dtype=torch.uint8).to(dev)
+    bufs = [torch.empty_like(buf) for _ in range(world)] if rank == root else None
+    dist.gather(buf, bufs, dst=root_global, group=group)
+    if rank != root:
+        return
+    images = [b[:n].cpu().numpy() for b, n in zip(bufs, sizes)]
+    if root == 0:
+        engine.merge_state(*images[1:])
+        return
+    # root's own state goes in its rank's place: start from nothing, and put it back if an image is refused
+    engine.reset()
+    try:
+        engine.merge_state(*images)
+    except Exception:
+        engine.merge_state(images[root])
+        raise

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define FPL_ABI_VERSION 9
+#define FPL_ABI_VERSION 10
 
 /* Filter result codes — identical to src/common.h:43-50 (they index FilterResult::mFilterReadStats[32]). */
 enum {
@@ -416,6 +416,55 @@ int fpl_allreduce_stats(fpl_ctx* ctx, int64_t cycles);
 int fpl_merge_stats(fpl_ctx* dst, fpl_ctx* const* src, int n_src);
 
 /*
+ * A context's accumulated state as one self-contained byte image, and images merged into a context — Stats::merge
+ * (src/stats.cpp:1013-1082) and FilterResult::merge (src/filterresult.cpp:28-61) for workers that are not contexts of this
+ * process on this device: shards processed on other GPUs, by other ranks or in other processes (array tasks over shard files,
+ * one engine per GPU) are merged into one context, which then writes the job's JSON and HTML reports.  The host carries the
+ * bytes (a file, torch.distributed with any backend, a socket).
+ *
+ * Image layout.  Little-endian (the library supports little-endian hosts only); int64 words unless said otherwise; every
+ * section starts on an 8-byte boundary and every padding byte is zero, so equal state gives equal bytes:
+ *   header, FPL_STATE_HEADER_BYTES:
+ *     words 0..14   FPL_STATE_MAGIC, FPL_STATE_FORMAT, FPL_ABI_VERSION, total bytes of the image,
+ *                   n_adapters, A = bytes of the adapter section, counter_words,
+ *                   rows = max(used_cycles, reduced_rows), used_cycles (the longest read accumulated),
+ *                   reduced_rows (the widest fpl_allreduce_stats), keep, complete, merged (the read lists' state, 0 or 1:
+ *                   capture on, every fpl_process_* call captured, all-reduced over several ranks), n_pre, n_post (entries
+ *                   of the two read lists in the image)
+ *     bytes 120..243  the fpl_options fields fpl_merge_stats compares but device (trim_front up to reserved), then 4 zero bytes
+ *   adapters, A bytes: per adapter in fpl_adapters order its length, then its bytes, zero-padded to a multiple of 8
+ *   Stats pre, then post, FPL_STATS_WORDS(rows) words each: rows [0, rows) of the 16 per-cycle arrays (array b, cycle c at
+ *     b * rows + c), then the tail
+ *   counters, counter_words words
+ *   read lists (fpl_keep_read_lists): n_pre, then n_post entries of 8 bytes (int32 length, int32 median char) — the entries
+ *     the context holds, none when capture was never on
+ *   total = FPL_STATE_HEADER_BYTES + A + 8 * (2 * FPL_STATS_WORDS(rows) + counter_words + n_pre + n_post)
+ * There is no checksum: the integrity of the transport is the caller's job.  Only images of this FPL_STATE_FORMAT and
+ * FPL_ABI_VERSION are read.
+ *
+ * fpl_state_export writes the image of ctx into host memory, behind everything queued on the context's stream.  Two phases:
+ * *n_bytes is always set; with out == NULL or cap < *n_bytes the call returns 1 and writes nothing.  Otherwise it returns 0
+ * with the image complete.  The context is not changed.
+ *
+ * fpl_state_merge leaves dst exactly as fpl_merge_stats(dst, {S1, ..., Sn}) would, Si being the context that exported image
+ * i: both Stats blocks, the counters, the longest read and the all-reduced width, the read lists (each image's entries
+ * appended in list order when dst keeps lists; otherwise dst's lists become incomplete), the complete / merged flags (so
+ * fpl_report_html refuses exactly what it refuses after fpl_merge_stats), and the built report texts invalidated.  Unlike
+ * fpl_merge_stats it ignores fpl_options.device and takes images from any process or device.  One k_merge_stats launch per
+ * call whatever the number of images.  Synchronous: the images may be released when it returns.
+ * Every image is validated on the host before dst changes, and nothing outside [images[i], images[i] + n_bytes[i]) is read.
+ * Refused (< 0, fpl_last_error, dst unchanged): a null dst, list or image, a negative count or size, a bad magic number,
+ * another format or ABI version, a size other than the header's (truncated, or trailing bytes), section lengths that do not
+ * add up, negative counts, flags other than 0 / 1, rows != max(used_cycles, reduced_rows), other options or another adapter
+ * list than dst's, another counter_words.  n_images == 0 does nothing.
+ */
+#define FPL_STATE_MAGIC 0x45544154534C5046ull   /* the bytes "FPLSTATE" */
+#define FPL_STATE_FORMAT 1
+#define FPL_STATE_HEADER_BYTES 248
+int fpl_state_export(fpl_ctx* ctx, uint8_t* out, int64_t cap, int64_t* n_bytes);
+int fpl_state_merge(fpl_ctx* dst, const uint8_t* const* images, const int64_t* n_bytes, int n_images);
+
+/*
  * SURVEY §8f row 4 — the counting half of Evaluator::evalAdapterAndReadNum (src/evaluator.cpp:105-265), context-free
  * because it runs before the adapters (and so the context) exist: over the reads of a HOST batch (the caller passes what
  * the reference would load: the first <= 64 Ki reads / 512 Mbases of the input) count the ten-mers of the first
@@ -461,7 +510,7 @@ int fpl_eval_pick_adapter(const uint32_t* counts, const uint64_t* position_acc, 
  *     with polyX trimming on
  * Two phases, like fpl_emit_fastq_host: *n_bytes is always set; with out == NULL or cap < *n_bytes the call returns 1 and
  * writes nothing — the text stays built on the device (for the same info), so a second call with room only copies.  Any later
- * call that changes the accumulators (fpl_process_*, fpl_reset, fpl_allreduce_stats, fpl_merge_stats into it, fpl_stats_reserve) invalidates the
+ * call that changes the accumulators (fpl_process_*, fpl_reset, fpl_allreduce_stats, fpl_merge_stats or fpl_state_merge into it, fpl_stats_reserve) invalidates the
  * built text; writes through fpl_stats_device_ptr / fpl_counters_device_ptr are not seen until one of those calls.
  * Synchronous.  Returns 0, 1, or < 0 on error.  The drop-in binary keeps the reference's own JsonReporter.
  */

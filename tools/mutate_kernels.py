@@ -10,8 +10,10 @@ changes no result by design), min / max ties, guards that cannot fire.
 the report / merge code: the rest of the battery calls none of fpl_report_json, fpl_report_html, fpl_merge_stats.
 --only ext runs only the --mask / --break cases, the only ones that reach fpl_ext.cu (fpl_ext_run runs only with one of the two
 flags on): the same verdict as the whole battery for a mutant of that file, in a fraction of the time.
-usage: python tools/mutate_kernels.py <file.cu> <n_mutants> [seed] [workers] [--range FROM[:TO]] [--only reports|ext]
-       (internal: --battery <lib.so|-> [<shrunk lib.so>] [reports|ext])"""
+--only state runs the in-process cases of tests/test_gpu_state.py, the only ones that call fpl_state_export / fpl_state_merge
+(its processes of their own, the gloo ranks and the cases past k_merge_stats' grid cap are left out).
+usage: python tools/mutate_kernels.py <file.cu> <n_mutants> [seed] [workers] [--range FROM[:TO]] [--only reports|ext|state]
+       (internal: --battery <lib.so|-> [<shrunk lib.so>] [reports|ext|state])"""
 import os
 import random
 import re
@@ -72,6 +74,22 @@ def ext_cases(T):
             T.check(opt, b, name)
 
 
+def state_cases():
+    """tests/test_gpu_state.py's cases that run in this process, on the mutant"""
+    import simt_emu
+    import test_gpu_state as S
+    from fastplong_b200 import binding
+    binding.LIB_PATH, binding._lib = simt_emu.build_library(), None
+    for name in sorted(S.M.SHARD_SETS):
+        S.test_round_trip(name)
+        S.test_shards_into_a_destination_holding_data(name)
+    for case in (S.test_source_longer_than_the_destination, S.test_destination_reserved_far_above,
+                 S.test_empty_sources_and_the_same_image_twice, S.test_capture_off, S.test_merged_flag_travels,
+                 S.test_processing_after_the_merge_continues_the_sequence,
+                 S.test_refusals_leave_the_destination_unchanged, S.test_two_phase_export, S.test_one_launch_per_merge):
+        case()
+
+
 def battery(lib, small=None, only=None):
     import signal
     import simt_emu
@@ -81,8 +99,12 @@ def battery(lib, small=None, only=None):
     import cases
     import test_capacity_shrunk as CS
     import test_simt_kernels as T
-    signal.alarm(300 if only in ("reports", "ext") else 900)       # the report cases take well under a minute
+    signal.alarm(300 if only in ("reports", "ext", "state") else 900)       # the report cases take well under a minute
     try:
+        if only == "state":
+            state_cases()
+            print("SURVIVED")
+            return
         if only == "reports":
             report_cases(small)
             print("SURVIVED")
@@ -167,7 +189,8 @@ def run_one(args):
     mutated = "\n".join(lines[:li] + [new] + lines[li + 1:])
     try:
         lib = simt_emu.build_library({fn: mutated}) if only != "reports" else "-"
-        small = simt_emu.build_library(capacity.shrunk_sources({fn: mutated}, **shrunk_values())) if only != "ext" else None
+        small = (simt_emu.build_library(capacity.shrunk_sources({fn: mutated}, **shrunk_values()))
+                 if only not in ("ext", "state") else None)
     except Exception:
         return k, "nocompile", lines[li], new
     try:
