@@ -17,6 +17,7 @@
 #include <cub/device/device_scan.cuh>
 #include "fpl_device.cuh"
 #include "fpl_scanplan.h"
+#include "fpl_scan.h"
 #include "fpl_stats.h"
 #include "fpl_jit.h"
 #include "fpl_ingest.h"
@@ -29,39 +30,6 @@ static_assert(sizeof(fpl_segment) == 20 && sizeof(fpl_region) == 12, "segment / 
 static_assert(sizeof(fpl_read_result) == 64, "fpl_read_result ABI size");
 static_assert(sizeof(ReadState) == 64, "ReadState size");
 static_assert(sizeof(StatSeg) == 24, "StatSeg size");
-
-#define QH_STRIPES 128      // stripes of k_scan_jit's histogram sums (fpl_scan_jit2_src.h)
-
-// kernel launchers (fpl_trim.cu, fpl_scan.cu, fpl_stats.cu)
-void launch_trim(const DevParams&, const DevBatch&, ReadState*, fpl_read_result*, unsigned long long*, cudaStream_t);
-void launch_scan(const DevParams&, const DevBatch&, ReadState*, cudaStream_t);
-void launch_scan_fast(const DevParams&, const ScanPlan&, const DevBatch&, ReadState*, cudaStream_t);
-void launch_final(const DevParams&, const DevBatch&, const ReadState*, fpl_read_result*, StatSeg*, int32_t*, int*, cudaStream_t);
-void launch_count(const fpl_read_result*, int64_t, unsigned long long*, bool, const int32_t*, unsigned long long*, unsigned long long*,
-                  int64_t, cudaStream_t);
-int launch_cycle_stats(CycleWs*, const uint8_t*, const uint8_t*, const StatSeg*, int64_t, int64_t, unsigned long long*, int64_t,
-                        bool, unsigned long long*, bool, const StatSeg*, unsigned long long*, const StatSeg*, cudaStream_t);
-void launch_kmer_fix(const DevBatch&, const fpl_read_result*, unsigned long long*, cudaStream_t);
-void launch_read_qual(const DevBatch&, unsigned long long*, unsigned long long*, int64_t, fpl_read_result*, bool, cudaStream_t);
-void launch_read_qual_exc(const DevBatch&, const ReadState*, const int32_t*, const int*, unsigned long long*, unsigned long long*, int64_t,
-                          fpl_read_result*, cudaStream_t);
-void launch_qhist_fold(const unsigned long long*, int, unsigned long long*, unsigned long long*, int64_t, cudaStream_t);
-void launch_make_preseg(const DevBatch&, StatSeg*, cudaStream_t);
-void launch_report_cycles(const unsigned long long*, const unsigned long long*, int64_t, unsigned long long*, cudaStream_t);
-void launch_report_sizes(const ReportCurves&, int64_t*, cudaStream_t);
-void launch_report_text(const ReportCurves&, const int64_t*, const uint8_t*, const int64_t*, const int64_t*, int, uint8_t*, cudaStream_t);
-void launch_html_capture(const fpl_read_result*, const int32_t*, int64_t, const fpl_segment*, int64_t, HtmlEntry*, HtmlEntry*, cudaStream_t);
-void launch_html_hist(const HtmlEntry*, int64_t, int64_t, long long*, cudaStream_t);
-void launch_html_scatter(const HtmlEntry*, int64_t, int64_t, const long long*, HtmlEntry*, cudaStream_t);
-void launch_html_lenhist(const HtmlEntry*, int64_t, unsigned long long*, cudaStream_t);
-void launch_html_lenprod(const unsigned long long*, int64_t, long long*, cudaStream_t);
-void launch_html_lensearch(const unsigned long long*, const long long*, const long long*, const long long*, int64_t, long long,
-                           unsigned long long, int*, cudaStream_t);
-void launch_html_bins(const unsigned long long*, int64_t, int64_t, unsigned long long*, cudaStream_t);
-void launch_html_values(const unsigned long long*, int64_t, int64_t, int, double*, cudaStream_t);
-void launch_html_sums(const double*, int64_t, const long long*, int64_t, double*, cudaStream_t);
-void launch_html_sizes(const HtmlText&, int64_t*, cudaStream_t);
-void launch_html_text(const HtmlText&, const int64_t*, const uint8_t*, const int64_t*, const int64_t*, int, uint8_t*, cudaStream_t);
 
 static thread_local char g_err[512] = "";
 
@@ -106,8 +74,26 @@ struct FplLists {
     bool merged = false;                // fpl_allreduce_stats over more than one rank since then
 };
 
+// The text of a report, kept in HBM until a call changes the accumulators (gen) or asks for other arguments (key), and what
+// places it: the sizes of its device-printed values and their exclusive sum, the frame pieces and their tables (frame_text)
+struct ReportText {
+    DevBuf<int64_t> d_size, d_off;
+    DevBuf<uint8_t> d_tmp, d_frame, d_text;
+    std::vector<uint8_t> h_frame;
+    int64_t n_bytes = 0;
+    std::string key;
+    int64_t gen = -1;                   // the accumulator generation of the text; -1: none
+};
+
+// fpl_report_json
+struct FplReport {
+    ReportText t;
+    DevBuf<unsigned long long> d_sum;   // k_report_cycles: total_cycles, bases, G+C of each block
+};
+
 // fpl_report_html: the text and its work buffers
 struct FplHtml {
+    ReportText t;
     DevBuf<HtmlEntry> d_grp[2];
     DevBuf<long long> d_mat;            // grouping histograms, then their exclusive sum in place
     DevBuf<long long> d_moff;
@@ -118,29 +104,6 @@ struct FplHtml {
     DevBuf<long long> d_x;
     DevBuf<double> d_vals;
     DevBuf<double> d_sums;
-    DevBuf<int64_t> d_size;
-    DevBuf<int64_t> d_off;
-    DevBuf<uint8_t> d_tmp;
-    DevBuf<uint8_t> d_frame;
-    DevBuf<uint8_t> d_text;
-    std::vector<uint8_t> h_frame;
-    bool built = false;
-    std::string key;
-    int64_t n_bytes = 0;
-};
-
-// fpl_report_json: the report text of the accumulators as they were when it was built, kept in HBM until a call changes them
-struct FplReport {
-    DevBuf<unsigned long long> d_sum;   // k_report_cycles: total_cycles, bases, G+C of each block
-    DevBuf<int64_t> d_size;             // bytes of every value
-    DevBuf<int64_t> d_off;              // their exclusive sum
-    DevBuf<uint8_t> d_tmp;
-    DevBuf<uint8_t> d_frame;            // piece tables + the host-built frame
-    DevBuf<uint8_t> d_text;
-    std::vector<uint8_t> h_frame;
-    bool built = false;
-    std::string key;                                // version, command and is_rna of the built text
-    int64_t n_bytes = 0;
 };
 
 // the context's NCCL communicator, released by ncclCommDestroy (defined where nccl() is)
@@ -217,6 +180,7 @@ struct fpl_ctx {
     // multi-GPU merge (fpl_comm_init / fpl_allreduce_stats): one NCCL communicator per context
     Owned<ncclComm_t, CommRelease> comm;
     int comm_rank = 0, comm_size = 1;
+    int64_t gen = 0;                    // accumulator generation: changes with the Stats, counters, flags or read lists
     int64_t used_cycles = 0;            // longest read accumulated since the last fpl_reset
     int64_t reduced_rows = 0;           // widest fpl_allreduce_stats since then: other ranks' reads may fill rows past used_cycles
     DevBuf<long long> d_agree;          // device word for the all-reduce(max) of the cycle count
@@ -251,7 +215,7 @@ static int ensure_reads(fpl_ctx* c, int64_t n) {
 // before they replace the old ones.
 static int reserve_cycles(fpl_ctx* c, int64_t need) {
     if (need <= c->C) return 0;
-    c->rep.built = false; c->html.built = false;
+    c->gen++;
     int64_t nc = c->C ? c->C : 1024;
     while (nc < need) nc *= 2;
     DevBuf<unsigned long long> nb[2];
@@ -298,15 +262,16 @@ static Event get_event(fpl_ctx* c) {
     return e;
 }
 
-// A launch timed when timing is on and both its events exist; without them it runs untimed.  It is counted either way.
+// The launches of one scope: timed as one launch of kernel k when timing is on and both its events exist (without them, or
+// with k < 0, they run untimed), and counted in fpl_launch_count by n, to which the launchers add the kernels they enqueue.
 struct Timed {
-    fpl_ctx* c; int k; bool ours; Event a, b;
-    Timed(fpl_ctx* c_, int k_, bool ours_ = true) : c(c_), k(k_), ours(ours_) {   // ours = false: a library kernel (NCCL), timed but not counted
-        if (c->timing) { a = get_event(c); b = get_event(c); }
+    fpl_ctx* c; int k; Event a, b; int n = 0;
+    Timed(fpl_ctx* c_, int k_) : c(c_), k(k_) {
+        if (c->timing && k >= 0) { a = get_event(c); b = get_event(c); }
         if (a && b) cudaEventRecord(a, c->stream);
     }
     ~Timed() {
-        if (ours) c->launches++;
+        c->launches += n;
         if (a && b) { cudaEventRecord(b, c->stream); c->events.push_back({k, std::move(a), std::move(b)}); }
     }
 };
@@ -351,7 +316,7 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
     collect_times(c);
     c->emit_valid = false; c->emit.built = false;
     c->bemit_valid = false; c->bemit.built = false;
-    c->rep.built = false; c->html.built = false;
+    c->gen++;
     c->bsrc = full;
     c->last_n = n;
     if (ensure_reads(c, n)) return -1;
@@ -405,61 +370,56 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
         StatSeg* pre = c->d_preseg + r0;
         StatSeg* post = c->d_postseg + 2 * r0;
         cudaStream_t s = c->stream;
-        { Timed t(c, K_PRESEG); launch_make_preseg(b, pre, s); }
-        { Timed t(c, K_TRIM); launch_trim(c->P, b, st, res, c->d_counters, s);
-          if (c->P.opt.adapter_enabled && c->n_adapters > 2) c->launches++; }   // + k_trim_fasta
+        { Timed t(c, K_PRESEG); launch_make_preseg(b, pre, s, t.n); }
+        { Timed t(c, K_TRIM); launch_trim(c->P, b, st, res, c->d_counters, s, t.n); }
         if (ext) {
             Timed t(c, K_CYCLE_PRE);
             if (launch_cycle_stats(&c->cycle_ws, full.seq, full.qual, pre, b.n_reads, tmax, c->d_stats[0], c->C, true, nullptr,
-                                   c->slots16, nullptr, nullptr, nullptr, s))
+                                   c->slots16, nullptr, nullptr, nullptr, s, t.n))
                 return fail("out of device memory (cycle stats workspace)");
-            c->launches += 2;   // + k_cs_keys and k_cs_gather around the (library) radix sort
         }
         {
             Timed t(c, K_SCAN);
-            if (c->jit.fn) { if (fpl_jit_launch_scan(&c->jit, b, st, s)) return fail("launching k_scan_jit failed"); }
-            else if (c->plan.fast) launch_scan_fast(c->P, c->plan, b, st, s);
-            else launch_scan(c->P, b, st, s);
+            if (c->jit.fn) { if (fpl_jit_launch_scan(&c->jit, b, st, s, t.n)) return fail("launching k_scan_jit failed"); }
+            else if (c->plan.fast) launch_scan_fast(c->P, c->plan, b, st, s, t.n);
+            else launch_scan(c->P, b, st, s, t.n);
         }
         int32_t* exc = qhist ? c->d_exc + r0 : nullptr;
         if (qhist) CK(cudaMemsetAsync(c->d_nexc, 0, sizeof(int), s));
-        { Timed t(c, K_FINAL); launch_final(c->P, b, st, res, post, exc, c->d_nexc, s); }
+        { Timed t(c, K_FINAL); launch_final(c->P, b, st, res, post, exc, c->d_nexc, s, t.n); }
         if (!ext) {
-            if (qhist) { Timed t(c, K_QUAL_EXC); launch_read_qual_exc(b, st, exc, c->d_nexc, c->d_stats[0], c->d_stats[1], c->C, res, s); }
+            if (qhist) { Timed t(c, K_QUAL_EXC); launch_read_qual_exc(b, st, exc, c->d_nexc, c->d_stats[0], c->d_stats[1], c->C, res, s, t.n); }
             { Timed t(c, K_COUNT);
-              launch_count(res, b.n_reads, c->d_counters, true, b.lens, qhist ? c->d_stats[0].get() : nullptr, c->d_stats[1], c->C, s); }
+              launch_count(res, b.n_reads, c->d_counters, true, b.lens, qhist ? c->d_stats[0].get() : nullptr, c->d_stats[1], c->C, s, t.n); }
             // one pass over the reads counts the pre-filter Stats and, for the read's slot-0 passing segment, the
             // post-filter per-cycle counters; the residual pass counts the passing segments it did not take
             { Timed t(c, K_CYCLE_PRE);
               if (launch_cycle_stats(&c->cycle_ws, full.seq, full.qual, pre, b.n_reads, tmax, c->d_stats[0], c->C, true,
-                                     c->d_stats[1] + 16 * c->C + FPL_STATS_KMER, c->slots16, post, c->d_stats[1], nullptr, s))
-                  return fail("out of device memory (cycle stats workspace)");
-              c->launches += 2; }   // + k_cs_keys and k_cs_gather around the (library) radix sort
+                                     c->d_stats[1] + 16 * c->C + FPL_STATS_KMER, c->slots16, post, c->d_stats[1], nullptr, s, t.n))
+                  return fail("out of device memory (cycle stats workspace)"); }
             { Timed t(c, K_CYCLE_POST);
               if (launch_cycle_stats(&c->cycle_ws, full.seq, full.qual, post, 2 * b.n_reads, tmax, c->d_stats[1], c->C, false, nullptr,
-                                     false, nullptr, nullptr, pre, s))
-                  return fail("out of device memory (cycle stats workspace)");
-              c->launches += 2; }   // + k_cs_keys and k_cs_gather around the (library) radix sort
-            { Timed t(c, K_KMER_FIX); launch_kmer_fix(b, res, c->d_stats[1] + 16 * c->C + FPL_STATS_KMER, s); }
-            if (!qhist) { Timed t(c, K_QUAL_PRE); launch_read_qual(b, c->d_stats[0], c->d_stats[1], c->C, res, false, s); }
+                                     false, nullptr, nullptr, pre, s, t.n))
+                  return fail("out of device memory (cycle stats workspace)"); }
+            { Timed t(c, K_KMER_FIX); launch_kmer_fix(b, res, c->d_stats[1] + 16 * c->C + FPL_STATS_KMER, s, t.n); }
+            if (!qhist) { Timed t(c, K_QUAL_PRE); launch_read_qual(b, c->d_stats[0], c->d_stats[1], c->C, res, false, s, t.n); }
         } else {
             // --mask / --break: k_final left the output reads of the adapter stage in the records; fpl_ext_run breaks /
             // masks / filters them (variable count) and the post-filter Stats run over its segment list
             char xerr[256] = "";
             const uint8_t* fseq = full.seq;
-            { Timed t(c, K_QUAL_PRE); launch_read_qual(b, c->d_stats[0], c->d_stats[1], c->C, res, true, s); }
-            { Timed t(c, K_COUNT); launch_count(res, b.n_reads, c->d_counters, false, nullptr, nullptr, nullptr, 0, s); }
+            { Timed t(c, K_QUAL_PRE); launch_read_qual(b, c->d_stats[0], c->d_stats[1], c->C, res, true, s, t.n); }
+            { Timed t(c, K_COUNT); launch_count(res, b.n_reads, c->d_counters, false, nullptr, nullptr, nullptr, 0, s, t.n); }
             if (fpl_ext_run(&c->ext, c->P, b, n_bytes, res, c->d_counters, c->d_stats[1], c->C, &fseq, s, xerr, sizeof(xerr)))
                 return fail("--mask/--break stage: %s", xerr);
             { Timed t(c, K_CYCLE_POST);
-              if (launch_cycle_stats(&c->cycle_ws, fseq, full.qual, c->ext.d_stat, c->ext.n_segs, tmax, c->d_stats[1], c->C, true, nullptr, false,
-                                     nullptr, nullptr, nullptr, s))
-                  return fail("out of device memory (cycle stats workspace)");
-          c->launches += 2; }   // + k_cs_keys and k_cs_gather around the (library) radix sort
+              if (launch_cycle_stats(&c->cycle_ws, fseq, full.qual, c->ext.d_stat, c->ext.n_segs, tmax, c->d_stats[1], c->C, true, nullptr,
+                                     false, nullptr, nullptr, nullptr, s, t.n))
+                  return fail("out of device memory (cycle stats workspace)"); }
         }
         r0 = r1;
     }
-    if (qhist && n > 0) { Timed t(c, K_QHIST_FOLD); launch_qhist_fold(c->d_qstripes, QH_STRIPES, c->d_stats[0], c->d_stats[1], c->C, c->stream); }
+    if (qhist && n > 0) { Timed t(c, K_QHIST_FOLD); launch_qhist_fold(c->d_qstripes, QH_STRIPES, c->d_stats[0], c->d_stats[1], c->C, c->stream, t.n); }
     if (c->lists.keep) {
         // after every kernel that writes a median: the call's entries behind the lists' ends.  Without --mask/--break the
         // post-filter list takes two slots per read (their segments), with them one per output read (ext.n_segs)
@@ -469,10 +429,9 @@ static int run_batch(fpl_ctx* c, const DevBatch& full, const int32_t* h_lens, fp
         if (n || n_post) {
             Timed t(c, K_HTML_CAPTURE);
             launch_html_capture(d_res, full.lens, n, ext ? c->ext.d_segs.get() : nullptr, ext ? n_post : 0, L.d[0] + L.n[0], L.d[1] + L.n[1],
-                                c->stream);
+                                c->stream, t.n);
         }
         L.n[0] += n; L.n[1] += n_post;
-        c->html.built = false;
     } else {
         c->lists.complete = false;
     }
@@ -854,8 +813,8 @@ int fpl_emit_fastq_host(fpl_ctx* c, int want_failed, uint8_t* out, int64_t out_c
         src.mseq = (c->P.opt.mask_enabled && c->ext.n_segs > 0) ? c->ext.d_mseq.get() : nullptr;   // fpl_ext_run made the masked copy
         src.offsets = c->ingest.d_offsets;
         char err[256] = "";
-        if (fpl_emit_build(&e, src, want_failed != 0, c->stream, err, sizeof(err))) return fail("fpl_emit_fastq_host: %s", err);
-        if (c->emit_n) c->launches += 2;
+        Timed t(c, -1);
+        if (fpl_emit_build(&e, src, want_failed != 0, c->stream, t.n, err, sizeof(err))) return fail("fpl_emit_fastq_host: %s", err);
     }
     *out_bytes = e.out_bytes;
     *failed_bytes = e.failed_bytes;
@@ -895,7 +854,7 @@ int fpl_emit_batch_device(fpl_ctx* c, fpl_out_batch* out, fpl_out_batch* failed)
         if (src.n_reads) {
             char err[256] = "";
             if (fpl_emit_batch_reserve(&e, src.n_reads, err, sizeof(err))) return fail("fpl_emit_batch_device: %s", err);
-            { Timed t(c, K_EMIT_BATCH_SIZES); launch_emit_batch_sizes(src, e.d_cnt, c->stream); }
+            { Timed t(c, K_EMIT_BATCH_SIZES); launch_emit_batch_sizes(src, e.d_cnt, c->stream, t.n); }
             if (fpl_emit_batch_scan(&e, src.n_reads, c->stream, err, sizeof(err))) return fail("fpl_emit_batch_device: %s", err);
         }
         e.built = true;
@@ -919,7 +878,7 @@ int fpl_emit_batch_device(fpl_ctx* c, fpl_out_batch* out, fpl_out_batch* failed)
         CK(cudaMemsetAsync(failed->seq + e.failed_bytes, 0, FPL_TAIL_PAD, c->stream));
         CK(cudaMemsetAsync(failed->qual + e.failed_bytes, 0, FPL_TAIL_PAD, c->stream));
     }
-    { Timed t(c, K_EMIT_BATCH_COPY); launch_emit_batch_copy(src, e.d_off, o, f, c->stream); }
+    { Timed t(c, K_EMIT_BATCH_COPY); launch_emit_batch_copy(src, e.d_off, o, f, c->stream, t.n); }
     CK(cudaGetLastError());
     return 0;
 }
@@ -1007,7 +966,7 @@ int fpl_reset(fpl_ctx* c) {
         CK(cudaMemsetAsync(c->d_stats[w], 0, sizeof(unsigned long long) * FPL_STATS_WORDS(c->C), c->stream));
     CK(cudaMemsetAsync(c->d_counters, 0, sizeof(unsigned long long) * c->counter_words, c->stream));
     c->used_cycles = 0; c->reduced_rows = 0;
-    c->rep.built = false; c->html.built = false;
+    c->gen++;
     c->lists.n[0] = c->lists.n[1] = 0;
     c->lists.complete = true; c->lists.merged = false;
     return 0;
@@ -1146,10 +1105,10 @@ int fpl_allreduce_stats(fpl_ctx* c, int64_t cycles) {
                                              (long long)cycles, (long long)c->used_cycles);
     // rows [b*C, b*C + cycles) of the 16 per-cycle arrays, then the tail; the row pointers depend on this rank's C, the
     // counts do not, so ranks need not share a capacity.  One group = one fused launch.
-    c->rep.built = false; c->html.built = false;
+    c->gen++;
     if (c->comm_size > 1) c->lists.merged = true;
     if (cycles > c->reduced_rows) c->reduced_rows = cycles;
-    Timed t(c, K_ALLREDUCE, false);
+    Timed t(c, K_ALLREDUCE);            // NCCL's kernels: timed, not counted
     CKN(nccl().GroupStart());
     for (int w = 0; w < 2; w++) {
         unsigned long long* blk = c->d_stats[w];
@@ -1314,24 +1273,88 @@ std::vector<std::string> report_frame(const fpl_options& o, const std::vector<st
     return p;
 }
 
-// the text of the accumulators as they are now, into c->rep
-int report_build(fpl_ctx* c, const char* version, const char* command, bool is_rna) {
-    FplReport& r = c->rep;
-    r.built = false;
+// k_report_cycles turns the first 6 words of d_sum (grown to `words`, all zero but the capacities in front of each block's
+// three) into total_cycles, bases and G+C of each block; those 6 words, both Stats tails and the counters come to the host
+int report_scalars(fpl_ctx* c, int k, DevBuf<unsigned long long>& d_sum, int64_t words, unsigned long long* sum,
+                   std::vector<long long>& tails, std::vector<long long>& cnt) {
     const int64_t C = c->C;
     cudaStream_t s = c->stream;
-    // 1. total_cycles, bases and G+C of both blocks; the tails and the counters come to the host
-    CK(r.d_sum.grow_exact(6));
-    unsigned long long sum[6] = {(unsigned long long)C, 0, 0, (unsigned long long)C, 0, 0};
-    CK(cudaMemcpyAsync(r.d_sum, sum, sizeof(sum), cudaMemcpyHostToDevice, s));
-    { Timed t(c, K_REPORT_CYCLES); launch_report_cycles(c->d_stats[0], c->d_stats[1], C, r.d_sum, s); }
-    std::vector<long long> tails(2 * FPL_STATS_TAIL), cnt((size_t)c->counter_words);
+    CK(d_sum.grow_exact(words));
+    std::vector<unsigned long long> init((size_t)words, 0);
+    init[0] = init[3] = (unsigned long long)C;
+    CK(cudaMemcpyAsync(d_sum, init.data(), sizeof(unsigned long long) * words, cudaMemcpyHostToDevice, s));
+    { Timed t(c, k); launch_report_cycles(c->d_stats[0], c->d_stats[1], C, d_sum, s, t.n); }
     for (int w = 0; w < 2; w++)
         CK(cudaMemcpyAsync(tails.data() + w * FPL_STATS_TAIL, c->d_stats[w] + 16 * C, sizeof(long long) * FPL_STATS_TAIL,
                            cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(cnt.data(), c->d_counters, sizeof(long long) * c->counter_words, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(sum, r.d_sum, sizeof(sum), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(sum, d_sum, 6 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
+    return 0;
+}
+
+// The frame pieces at their places around the device-printed gaps, piece j in front of gap j and the last behind them all;
+// gap j ends where t.d_off[at[j]] says.  Sets shift[j], the frame bytes in front of gap j, uploads the source / destination
+// tables and the pieces, and launch(pieces, src, dst, n_pieces, launched) prints the text into t.d_text, timed as kernel k.
+template <class Launch>
+int frame_text(fpl_ctx* c, ReportText& t, int k, const std::vector<std::string>& frame, const std::vector<int64_t>& at, int64_t* shift,
+               Launch&& launch) {
+    const int np = (int)frame.size();
+    std::vector<int64_t> end(np - 1), src(np + 1, 0), dst(np);
+    for (int j = 0; j + 1 < np; j++)
+        CK(cudaMemcpyAsync(&end[j], t.d_off + at[j], sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    for (int j = 0; j < np; j++) {
+        src[j + 1] = src[j] + (int64_t)frame[j].size();
+        dst[j] = (j ? end[j - 1] : 0) + src[j];         // behind gap j - 1
+        if (j + 1 < np) shift[j] = src[j + 1];
+    }
+    const int64_t total = end[np - 2] + src[np];
+    const size_t tables = sizeof(int64_t) * (2 * np + 1);
+    t.h_frame.resize(tables + (size_t)src[np]);
+    memcpy(t.h_frame.data(), src.data(), sizeof(int64_t) * (np + 1));
+    memcpy(t.h_frame.data() + sizeof(int64_t) * (np + 1), dst.data(), sizeof(int64_t) * np);
+    for (int j = 0; j < np; j++) memcpy(t.h_frame.data() + tables + src[j], frame[j].data(), frame[j].size());
+    CK(t.d_frame.grow((int64_t)t.h_frame.size()));
+    CK(t.d_text.grow(total));
+    CK(cudaMemcpyAsync(t.d_frame, t.h_frame.data(), t.h_frame.size(), cudaMemcpyHostToDevice, c->stream));
+    {
+        Timed tm(c, k);
+        const int64_t* d_src = reinterpret_cast<const int64_t*>(t.d_frame.get());
+        launch(t.d_frame + tables, d_src, d_src + np + 1, np, tm.n);
+    }
+    CK(cudaGetLastError());
+    t.n_bytes = total;
+    return 0;
+}
+
+// Both entry points' two-phase copy-out: the text for `key` of the accumulators as they are, kept from an earlier call or
+// made by build(); 1 (with *n_bytes) when out cannot take it, and the text stays for the call that can
+template <class Build>
+int report_out(fpl_ctx* c, ReportText& t, std::string key, Build&& build, uint8_t* out, int64_t cap, int64_t* n_bytes) {
+    CK(cudaSetDevice(c->device));
+    if (t.gen != c->gen || t.key != key) {
+        t.gen = -1;                     // a build that fails leaves no text
+        if (build()) return -1;
+        t.key.swap(key);
+        t.gen = c->gen;
+    }
+    *n_bytes = t.n_bytes;
+    if (!out || cap < t.n_bytes) return 1;
+    CK(cudaMemcpyAsync(out, t.d_text, (size_t)t.n_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    collect_times(c);
+    return 0;
+}
+
+// the JSON text of the accumulators as they are now, into c->rep.t
+int report_build(fpl_ctx* c, const char* version, const char* command, bool is_rna) {
+    const int64_t C = c->C;
+    cudaStream_t s = c->stream;
+    // 1. total_cycles, bases and G+C of both blocks; the tails and the counters
+    unsigned long long sum[6];
+    std::vector<long long> tails(2 * FPL_STATS_TAIL), cnt((size_t)c->counter_words);
+    if (report_scalars(c, K_REPORT_CYCLES, c->rep.d_sum, 6, sum, tails, cnt)) return -1;
     RepBlock b[2];
     for (int w = 0; w < 2; w++) {
         const long long* tl = tails.data() + w * FPL_STATS_TAIL;
@@ -1343,52 +1366,21 @@ int report_build(fpl_ctx* c, const char* version, const char* command, bool is_r
     }
     const std::vector<std::string> frame = report_frame(c->P.opt, c->adapter_str, cnt.data(), b, version, command, is_rna);
     // 2. the size of every value, their exclusive sum (the n + 1st entry: the curves' total)
+    ReportText& x = c->rep.t;
     ReportCurves R = {};
     R.blk[0] = c->d_stats[0]; R.blk[1] = c->d_stats[1]; R.C = C; R.T[0] = b[0].cycles; R.T[1] = b[1].cycles;
     R.is_rna = is_rna ? 1 : 0;
     const int64_t n = 11 * (R.T[0] + R.T[1]);
-    CK(r.d_size.grow(n + 1));
-    CK(r.d_off.grow(n + 1));
-    CK(cudaMemsetAsync(r.d_size + n, 0, sizeof(int64_t), s));
-    { Timed t(c, K_REPORT_SIZES); launch_report_sizes(R, r.d_size, s); }
-    CK(cub_call(r.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, r.d_size.get(), r.d_off.get(), n + 1, s); }));
-    int64_t end[22];                   // the running sum behind curve j
-    for (int j = 0; j < 22; j++) {
-        const int w = j / 11, k = j % 11;
-        CK(cudaMemcpyAsync(&end[j], r.d_off + (w ? 11 * R.T[0] : 0) + (int64_t)(k + 1) * R.T[w], sizeof(int64_t),
-                           cudaMemcpyDeviceToHost, s));
-    }
-    CK(cudaStreamSynchronize(s));
+    CK(x.d_size.grow(n + 1));
+    CK(x.d_off.grow(n + 1));
+    CK(cudaMemsetAsync(x.d_size + n, 0, sizeof(int64_t), s));
+    { Timed t(c, K_REPORT_SIZES); launch_report_sizes(R, x.d_size, s, t.n); }
+    CK(cub_call(x.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, x.d_size.get(), x.d_off.get(), n + 1, s); }));
+    std::vector<int64_t> at(22);       // curve j ends at value 11 * T[0] * w + (k + 1) * T[w], w = j / 11, k = j % 11
+    for (int j = 0; j < 22; j++) at[j] = (j < 11 ? 0 : 11 * R.T[0]) + (int64_t)(j % 11 + 1) * R.T[j / 11];
     // 3. the frame pieces at their places, the curves between them
-    std::vector<int64_t> src(24), dst(23);
-    int64_t fbytes = 0, shift = 0;
-    for (int j = 0; j < 23; j++) {
-        src[j] = fbytes;
-        dst[j] = (j ? end[j - 1] : 0) + shift;      // behind curve j - 1
-        shift += (int64_t)frame[j].size();
-        fbytes += (int64_t)frame[j].size();
-        if (j < 22) R.shift[j] = shift;
-    }
-    src[23] = fbytes;
-    const int64_t total = end[21] + shift;
-    const size_t tables = sizeof(int64_t) * (24 + 23);
-    r.h_frame.resize(tables + (size_t)fbytes);
-    memcpy(r.h_frame.data(), src.data(), sizeof(int64_t) * 24);
-    memcpy(r.h_frame.data() + sizeof(int64_t) * 24, dst.data(), sizeof(int64_t) * 23);
-    for (int j = 0; j < 23; j++) memcpy(r.h_frame.data() + tables + src[j], frame[j].data(), frame[j].size());
-    CK(r.d_frame.grow((int64_t)r.h_frame.size()));
-    CK(r.d_text.grow(total));
-    CK(cudaMemcpyAsync(r.d_frame, r.h_frame.data(), r.h_frame.size(), cudaMemcpyHostToDevice, s));
-    {
-        Timed t(c, K_REPORT_TEXT);
-        const int64_t* d_src = reinterpret_cast<const int64_t*>(r.d_frame.get());
-        launch_report_text(R, r.d_off, r.d_frame + tables, d_src, d_src + 24, 23, r.d_text, s);
-        c->launches++;                 // + k_report_frame
-    }
-    CK(cudaGetLastError());
-    r.n_bytes = total;
-    r.built = true;
-    return 0;
+    return frame_text(c, x, K_REPORT_TEXT, frame, at, R.shift, [&](const uint8_t* pieces, const int64_t* src, const int64_t* dst, int np,
+                                                                   int& n) { launch_report_text(R, x.d_off, pieces, src, dst, np, x.d_text, s, n); });
 }
 
 }  // namespace
@@ -1400,18 +1392,9 @@ extern "C" int fpl_report_json(fpl_ctx* c, const fpl_report_info* info, uint8_t*
     if (info->struct_size != (int32_t)sizeof(fpl_report_info))
         return fail("fpl_report_json: fpl_report_info.struct_size %d != %d (ABI mismatch)", info->struct_size, (int)sizeof(fpl_report_info));
     if (!info->version || !info->command) return fail("fpl_report_json: version and command must not be null");
-    CK(cudaSetDevice(c->device));
-    std::string key = std::string(info->version) + '\0' + info->command + '\0' + (info->is_rna ? "U" : "T");
-    if (!c->rep.built || c->rep.key != key) {
-        if (report_build(c, info->version, info->command, info->is_rna != 0)) { c->rep.built = false; return -1; }
-        c->rep.key.swap(key);
-    }
-    *n_bytes = c->rep.n_bytes;
-    if (!out || cap < c->rep.n_bytes) return 1;     // the text stays built: call again with room
-    CK(cudaMemcpyAsync(out, c->rep.d_text, (size_t)c->rep.n_bytes, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    collect_times(c);
-    return 0;
+    const std::string key = std::string(info->version) + '\0' + info->command + '\0' + (info->is_rna ? "U" : "T");
+    return report_out(c, c->rep.t, key, [&] { return report_build(c, info->version, info->command, info->is_rna != 0); }, out, cap,
+                      n_bytes);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1779,28 +1762,19 @@ std::vector<std::string> html_frame(const fpl_options& o, const long long* cnt, 
 
 int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
     FplHtml& h = c->html;
+    ReportText& x = h.t;
     FplLists& L = c->lists;
-    h.built = false;
     const int64_t C = c->C;
     cudaStream_t s = c->stream;
-    // 1. total_cycles, bases and G+C (k_report_cycles), then the base-bin counts below total_cycles
-    CK(h.d_sum.grow_exact(22));
-    CK(h.d_lstat.grow_exact(8));
-    unsigned long long sum[22] = {(unsigned long long)C, 0, 0, (unsigned long long)C, 0, 0};
-    CK(cudaMemcpyAsync(h.d_sum, sum, sizeof(sum), cudaMemcpyHostToDevice, s));
-    { Timed t(c, K_HTML_CYCLES); launch_report_cycles(c->d_stats[0], c->d_stats[1], C, h.d_sum, s); }
+    // 1. total_cycles, bases and G+C, the tails and the counters, then the base-bin counts below total_cycles
+    unsigned long long sum[22];
     std::vector<long long> tails(2 * FPL_STATS_TAIL), cnt((size_t)c->counter_words);
-    for (int w = 0; w < 2; w++)
-        CK(cudaMemcpyAsync(tails.data() + w * FPL_STATS_TAIL, c->d_stats[w] + 16 * C, sizeof(long long) * FPL_STATS_TAIL,
-                           cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(cnt.data(), c->d_counters, sizeof(long long) * c->counter_words, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(sum, h.d_sum, 6 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    if (report_scalars(c, K_HTML_CYCLES, h.d_sum, 22, sum, tails, cnt)) return -1;
+    CK(h.d_lstat.grow_exact(8));
     const int64_t T[2] = {(int64_t)sum[0], (int64_t)sum[3]};
     {
         Timed t(c, K_HTML_CYCLES);
-        for (int w = 0; w < 2; w++) launch_html_bins(c->d_stats[w], C, T[w], h.d_sum + 6 + 8 * w, s);
-        c->launches += (T[0] > 0) + (T[1] > 0) - 1;  // one k_html_bins per block with cycles
+        for (int w = 0; w < 2; w++) launch_html_bins(c->d_stats[w], C, T[w], h.d_sum + 6 + 8 * w, s, t.n);
     }
     // 2. each list grouped by median: the entries of bins 0..127 are the density pairs, bin 128 the empty reads
     int64_t M[2] = {0, 0}, NE[2] = {0, 0};
@@ -1812,9 +1786,9 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
         CK(h.d_moff.grow(m));
         CK(h.d_grp[w].grow(n));
         CK(cudaMemsetAsync(h.d_mat + m - 1, 0, sizeof(long long), s));
-        { Timed t(c, K_HTML_GROUP_HIST); launch_html_hist(L.d[w], n, nch, h.d_mat, s); }
-        CK(cub_call(h.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, h.d_mat.get(), h.d_moff.get(), m, s); }));
-        { Timed t(c, K_HTML_GROUP_SCATTER); launch_html_scatter(L.d[w], n, nch, h.d_moff, h.d_grp[w], s); }
+        { Timed t(c, K_HTML_GROUP_HIST); launch_html_hist(L.d[w], n, nch, h.d_mat, s, t.n); }
+        CK(cub_call(x.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, h.d_mat.get(), h.d_moff.get(), m, s); }));
+        { Timed t(c, K_HTML_GROUP_SCATTER); launch_html_scatter(L.d[w], n, nch, h.d_moff, h.d_grp[w], s, t.n); }
         CK(cudaMemcpyAsync(&NE[w], h.d_moff + 128 * nch, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(&M[w], h.d_moff + 129 * nch, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
@@ -1830,13 +1804,12 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
         unsigned long long* hist = h.d_hist + w * H;
         long long *ccum = h.d_lwork + 3 * w * H, *prod = ccum + H, *pcum = prod + H;
         Timed t(c, K_HTML_LENGTHS);
-        launch_html_lenhist(L.d[w], L.n[w], hist, s);
-        launch_html_lenprod(hist, H, prod, s);
-        CK(cub_call(h.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, hist, ccum, H, s); }));
-        CK(cub_call(h.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, prod, pcum, H, s); }));
+        launch_html_lenhist(L.d[w], L.n[w], hist, s, t.n);
+        launch_html_lenprod(hist, H, prod, s, t.n);
+        CK(cub_call(x.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, hist, ccum, H, s); }));
+        CK(cub_call(x.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, prod, pcum, H, s); }));
         const long long lensum = tails[w * FPL_STATS_TAIL + FPL_STATS_LENSUM];
-        launch_html_lensearch(hist, ccum, prod, pcum, H, lensum / 2, (unsigned long long)M[w] / 2, h.d_lstat + 4 * w, s);
-        c->launches += L.n[w] ? 2 : 1;               // k_html_lenhist (with entries), k_html_lenprod, k_html_lensearch
+        launch_html_lensearch(hist, ccum, prod, pcum, H, lensum / 2, (unsigned long long)M[w] / 2, h.d_lstat + 4 * w, s, t.n);
     }
     int lstat[8];
     CK(cudaMemcpyAsync(lstat, h.d_lstat, sizeof(lstat), cudaMemcpyDeviceToHost, s));
@@ -1869,8 +1842,8 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
     if (!xs.empty()) CK(cudaMemcpyAsync(h.d_x, xs.data(), sizeof(long long) * xs.size(), cudaMemcpyHostToDevice, s));
     for (int w = 0; w < 2; w++) {
         double* vals = h.d_vals + (w ? 11 * T[0] : 0);
-        if (T[w]) { Timed t(c, K_HTML_VALUES); launch_html_values(c->d_stats[w], C, T[w], info.is_rna != 0, vals, s); }
-        if (R[w]) { Timed t(c, K_HTML_SUMS); launch_html_sums(vals, T[w], h.d_x + (w ? R[0] : 0), R[w], h.d_sums + (w ? 11 * R[0] : 0), s); }
+        if (T[w]) { Timed t(c, K_HTML_VALUES); launch_html_values(c->d_stats[w], C, T[w], info.is_rna != 0, vals, s, t.n); }
+        if (R[w]) { Timed t(c, K_HTML_SUMS); launch_html_sums(vals, T[w], h.d_x + (w ? R[0] : 0), R[w], h.d_sums + (w ? 11 * R[0] : 0), s, t.n); }
     }
     // 5. the frame, the size of every value and their exclusive sum
     const std::vector<std::string> frame = html_frame(c->P.opt, cnt.data(), b, info);
@@ -1897,46 +1870,15 @@ int html_build(fpl_ctx* c, const fpl_report_html_info& info) {
         X.sums[w] = h.d_sums + (w ? 11 * R[0] : 0);
         X.x[w] = h.d_x + (w ? R[0] : 0);
     }
-    CK(h.d_size.grow(items + 1));
-    CK(h.d_off.grow(items + 1));
-    CK(cudaMemsetAsync(h.d_size + items, 0, sizeof(int64_t), s));
-    if (items) { Timed t(c, K_HTML_SIZES); launch_html_sizes(X, h.d_size, s); }
-    CK(cub_call(h.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, h.d_size.get(), h.d_off.get(), items + 1, s); }));
-    int64_t end[HTML_SEGS];            // the running sum behind segment j
-    for (int j = 0; j < HTML_SEGS; j++)
-        CK(cudaMemcpyAsync(&end[j], h.d_off + X.start[j + 1], sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    // 6. the frame pieces at their places, the values between them
-    const int np = HTML_SEGS + 1;
-    std::vector<int64_t> src(np + 1), dst(np);
-    int64_t fbytes = 0, shift = 0;
-    for (int j = 0; j < np; j++) {
-        src[j] = fbytes;
-        dst[j] = (j ? end[j - 1] : 0) + shift;
-        shift += (int64_t)frame[j].size();
-        fbytes += (int64_t)frame[j].size();
-        if (j < HTML_SEGS) X.shift[j] = shift;
-    }
-    src[np] = fbytes;
-    const int64_t total = end[HTML_SEGS - 1] + shift;
-    const size_t tables = sizeof(int64_t) * (2 * np + 1);
-    h.h_frame.resize(tables + (size_t)fbytes);
-    memcpy(h.h_frame.data(), src.data(), sizeof(int64_t) * (np + 1));
-    memcpy(h.h_frame.data() + sizeof(int64_t) * (np + 1), dst.data(), sizeof(int64_t) * np);
-    for (int j = 0; j < np; j++) memcpy(h.h_frame.data() + tables + src[j], frame[j].data(), frame[j].size());
-    CK(h.d_frame.grow((int64_t)h.h_frame.size()));
-    CK(h.d_text.grow(total));
-    CK(cudaMemcpyAsync(h.d_frame, h.h_frame.data(), h.h_frame.size(), cudaMemcpyHostToDevice, s));
-    {
-        Timed t(c, K_HTML_TEXT);
-        const int64_t* d_src = reinterpret_cast<const int64_t*>(h.d_frame.get());
-        launch_html_text(X, h.d_off, h.d_frame + tables, d_src, d_src + np + 1, np, h.d_text, s);
-        if (items) c->launches++;      // k_report_frame + k_html_text (only with values to print)
-    }
-    CK(cudaGetLastError());
-    h.n_bytes = total;
-    h.built = true;
-    return 0;
+    CK(x.d_size.grow(items + 1));
+    CK(x.d_off.grow(items + 1));
+    CK(cudaMemsetAsync(x.d_size + items, 0, sizeof(int64_t), s));
+    if (items) { Timed t(c, K_HTML_SIZES); launch_html_sizes(X, x.d_size, s, t.n); }
+    CK(cub_call(x.d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, x.d_size.get(), x.d_off.get(), items + 1, s); }));
+    // 6. the frame pieces at their places, the values between them (segment j ends where segment j + 1 starts)
+    const std::vector<int64_t> at(X.start + 1, X.start + HTML_SEGS + 1);
+    return frame_text(c, x, K_HTML_TEXT, frame, at, X.shift, [&](const uint8_t* pieces, const int64_t* src, const int64_t* dst, int np,
+                                                                 int& n) { launch_html_text(X, x.d_off, pieces, src, dst, np, x.d_text, s, n); });
 }
 
 }  // namespace
@@ -1962,19 +1904,9 @@ extern "C" int fpl_report_html(fpl_ctx* c, const fpl_report_html_info* info, uin
                     "or fpl_reset: the lists are incomplete");
     if (c->lists.merged)
         return fail("fpl_report_html: fpl_allreduce_stats merged the Stats over several ranks, but not the read lists");
-    CK(cudaSetDevice(c->device));
-    std::string key = std::string(info->version) + '\0' + info->command + '\0' + info->title + '\0' + info->time_text + '\0' +
-                      (info->is_rna ? "U" : "T");
-    if (!c->html.built || c->html.key != key) {
-        if (html_build(c, *info)) { c->html.built = false; return -1; }
-        c->html.key.swap(key);
-    }
-    *n_bytes = c->html.n_bytes;
-    if (!out || cap < c->html.n_bytes) return 1;     // the text stays built: call again with room
-    CK(cudaMemcpyAsync(out, c->html.d_text, (size_t)c->html.n_bytes, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    collect_times(c);
-    return 0;
+    const std::string key = std::string(info->version) + '\0' + info->command + '\0' + info->title + '\0' + info->time_text + '\0' +
+                            (info->is_rna ? "U" : "T");
+    return report_out(c, c->html.t, key, [&] { return html_build(c, *info); }, out, cap, n_bytes);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1982,6 +1914,62 @@ extern "C" int fpl_report_html(fpl_ctx* c, const fpl_report_html_info* info, uin
 // src/seprocessor.cpp:108-121).  The accumulators are summed by k_merge_stats, the read lists appended by device copies; all of
 // it on dst's stream, between an event wait on every source's stream and a wait of every source's stream on dst's.
 // ------------------------------------------------------------------------------------------------------------------
+namespace {
+
+// One source of a merge: its accumulators as k_merge_stats reads them (src.rows: the rows that may hold counts), its flags
+// and list lengths, and its list entries (device memory for a context, host memory for a state image)
+struct MergeIn {
+    MergeSrc src;
+    int64_t used, reduced, n[2];
+    bool complete, merged;
+    const void* list[2];
+};
+
+// fpl_merge_stats / fpl_state_merge with their sources, in order: the capacities reserved, stage() (c's stream behind the
+// sources, or their accumulators staged on the device), one k_merge_stats, the list entries appended behind c's by copies of
+// `kind`, and the combined rows, flags and lengths committed.  A failure before the launch leaves c as it was.
+template <class Stage>
+int merge_core(fpl_ctx* c, const std::vector<MergeIn>& in, cudaMemcpyKind kind, Stage&& stage) {
+    FplLists& L = c->lists;
+    int64_t rows = 0, used = c->used_cycles, reduced = c->reduced_rows, total[2] = {L.n[0], L.n[1]};
+    bool complete = L.complete, merged = L.merged;
+    for (const MergeIn& s : in) {
+        rows = std::max(rows, s.src.rows);
+        used = std::max(used, s.used);
+        reduced = std::max(reduced, s.reduced);
+        complete = complete && s.complete;
+        merged = merged || s.merged;
+        for (int w = 0; w < 2; w++) total[w] += s.n[w];
+    }
+    // the capacities first: they synchronise c's stream when they grow
+    if (reserve_cycles(c, rows)) return -1;
+    if (L.keep && (grow_list(c, 0, total[0]) || grow_list(c, 1, total[1]))) return -1;
+    if (stage()) return -1;
+    const int n_src = (int)in.size();
+    std::vector<MergeSrc> tab;
+    for (const MergeIn& s : in) tab.push_back(s.src);
+    CK(c->d_merge.grow(n_src));
+    CK(cudaMemcpyAsync(c->d_merge, tab.data(), sizeof(MergeSrc) * n_src, cudaMemcpyHostToDevice, c->stream));
+    { Timed t(c, K_MERGE_STATS);
+      launch_merge_stats(c->d_stats[0], c->d_stats[1], c->d_counters, c->C, rows, c->counter_words, c->d_merge, n_src, c->stream, t.n); }
+    if (L.keep) {
+        for (int w = 0; w < 2; w++)
+            for (const MergeIn& s : in) {
+                if (s.n[w]) CK(cudaMemcpyAsync(L.d[w] + L.n[w], s.list[w], sizeof(HtmlEntry) * s.n[w], kind, c->stream));
+                L.n[w] += s.n[w];
+            }
+    } else {
+        complete = false;                     // the sources' entries were not taken, as in a call with capture off
+    }
+    c->used_cycles = used; c->reduced_rows = reduced;
+    L.complete = complete; L.merged = merged;
+    c->gen++;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+}  // namespace
+
 extern "C" int fpl_merge_stats(fpl_ctx* c, fpl_ctx* const* src, int n_src) {
     g_err[0] = 0;
     if (!c) return fail("fpl_merge_stats: null destination context");
@@ -2003,54 +1991,24 @@ extern "C" int fpl_merge_stats(fpl_ctx* c, fpl_ctx* const* src, int n_src) {
     }
     if (n_src == 0) return 0;
     CK(cudaSetDevice(c->device));
-    FplLists& L = c->lists;
-    int64_t rows = 0, used = c->used_cycles, reduced = c->reduced_rows, total[2] = {L.n[0], L.n[1]};
-    bool complete = L.complete, merged = L.merged;
-    std::vector<MergeSrc> tab((size_t)n_src);
+    std::vector<MergeIn> in((size_t)n_src);
     for (int k = 0; k < n_src; k++) {
         const fpl_ctx* s = src[k];
-        const int64_t r = std::max(s->used_cycles, s->reduced_rows);
-        tab[k] = MergeSrc{{s->d_stats[0], s->d_stats[1]}, s->d_counters, s->C, r};
-        rows = std::max(rows, r);
-        used = std::max(used, s->used_cycles);
-        reduced = std::max(reduced, s->reduced_rows);
-        complete = complete && s->lists.complete;
-        merged = merged || s->lists.merged;
-        for (int w = 0; w < 2; w++) total[w] += s->lists.n[w];
+        const FplLists& S = s->lists;
+        in[k] = MergeIn{MergeSrc{{s->d_stats[0], s->d_stats[1]}, s->d_counters, s->C, std::max(s->used_cycles, s->reduced_rows)},
+                        s->used_cycles, s->reduced_rows, {S.n[0], S.n[1]}, S.complete, S.merged, {S.d[0], S.d[1]}};
     }
-    // the capacities first: they synchronise dst's stream when they grow
-    if (reserve_cycles(c, rows)) return -1;
-    if (L.keep && (grow_list(c, 0, total[0]) || grow_list(c, 1, total[1]))) return -1;
-    CK(c->d_merge.grow(n_src));
-    if (!c->merge_ev) CK(create_event(c->merge_ev, false));
-    for (int k = 0; k < n_src; k++) {         // behind everything queued on the sources
-        CK(cudaEventRecord(c->merge_ev, src[k]->stream));
-        CK(cudaStreamWaitEvent(c->stream, c->merge_ev, 0));
-    }
-    CK(cudaMemcpyAsync(c->d_merge, tab.data(), sizeof(MergeSrc) * n_src, cudaMemcpyHostToDevice, c->stream));
-    {
-        Timed t(c, K_MERGE_STATS);
-        launch_merge_stats(c->d_stats[0], c->d_stats[1], c->d_counters, c->C, rows, c->counter_words, c->d_merge, n_src, c->stream);
-    }
-    if (L.keep) {
-        for (int w = 0; w < 2; w++) {
-            int64_t at = L.n[w];
-            for (int k = 0; k < n_src; k++) {
-                const int64_t n = src[k]->lists.n[w];
-                if (n) CK(cudaMemcpyAsync(L.d[w] + at, src[k]->lists.d[w], sizeof(HtmlEntry) * n, cudaMemcpyDeviceToDevice, c->stream));
-                at += n;
-            }
-            L.n[w] = at;
+    auto behind_sources = [&] {               // behind everything queued on the sources
+        if (!c->merge_ev) CK(create_event(c->merge_ev, false));
+        for (int k = 0; k < n_src; k++) {
+            CK(cudaEventRecord(c->merge_ev, src[k]->stream));
+            CK(cudaStreamWaitEvent(c->stream, c->merge_ev, 0));
         }
-    } else {
-        complete = false;                     // the sources' entries were not captured, as in a call with capture off
-    }
+        return 0;
+    };
+    if (merge_core(c, in, cudaMemcpyDeviceToDevice, behind_sources)) return -1;
     CK(cudaEventRecord(c->merge_ev, c->stream));
     for (int k = 0; k < n_src; k++) CK(cudaStreamWaitEvent(src[k]->stream, c->merge_ev, 0));   // before the sources' next work
-    c->used_cycles = used; c->reduced_rows = reduced;
-    L.complete = complete; L.merged = merged;
-    c->rep.built = false; c->html.built = false;
-    CK(cudaGetLastError());
     return 0;
 }
 
@@ -2083,16 +2041,10 @@ int64_t adapter_section_bytes(const std::vector<std::string>& a) {
     return n;
 }
 
-// one validated image: its flags, list lengths and where its sections are
-struct StateImage {
-    int64_t rows, used, reduced, n[2];
-    bool complete, merged;
-    const uint8_t* stats;                   // pre and post Stats, then the counters: contiguous
-    const uint8_t* list[2];
-};
-
-// Validation of image i against dst, on the host, reading nothing outside [p, p + n)
-int parse_image(const fpl_ctx* c, int i, const uint8_t* p, int64_t n, StateImage& im) {
+// Validation of image i against dst, on the host, reading nothing outside [p, p + n): its merge source, whose MergeSrc has
+// capacity and rows `rows` and no addresses yet, and its Stats and counter sections (pre and post Stats, then the counters:
+// contiguous)
+int parse_image(const fpl_ctx* c, int i, const uint8_t* p, int64_t n, MergeIn& im, const uint8_t*& stats) {
     if (!p) return fail("fpl_state_merge: image %d is null", i);
     if (n < 0) return fail("fpl_state_merge: image %d has a negative size (%lld)", i, (long long)n);
     if (n < FPL_STATE_HEADER_BYTES)
@@ -2136,12 +2088,10 @@ int parse_image(const fpl_ctx* c, int i, const uint8_t* p, int64_t n, StateImage
     if (cw != c->counter_words)
         return fail("fpl_state_merge: image %d has %lld counter words, the destination %lld", i, (long long)cw,
                     (long long)c->counter_words);
-    im.rows = rows; im.used = h[SI_USED]; im.reduced = h[SI_REDUCED];
-    im.n[0] = n0; im.n[1] = n1;
-    im.complete = h[SI_COMPLETE] != 0; im.merged = h[SI_MERGED] != 0;
-    im.stats = q;
-    im.list[0] = q + 8 * (2 * FPL_STATS_WORDS(rows) + cw);
-    im.list[1] = im.list[0] + 8 * n0;
+    const uint8_t* list = q + 8 * (2 * FPL_STATS_WORDS(rows) + cw);
+    im = MergeIn{MergeSrc{{nullptr, nullptr}, nullptr, rows, rows}, h[SI_USED], h[SI_REDUCED], {n0, n1}, h[SI_COMPLETE] != 0,
+                 h[SI_MERGED] != 0, {list, list + 8 * n0}};
+    stats = q;
     return 0;
 }
 
@@ -2193,58 +2143,29 @@ extern "C" int fpl_state_merge(fpl_ctx* c, const uint8_t* const* images, const i
     if (!c) return fail("fpl_state_merge: null destination context");
     if (n_images < 0) return fail("fpl_state_merge: negative number of images (%d)", n_images);
     if (n_images > 0 && (!images || !n_bytes)) return fail("fpl_state_merge: null image or size list");
-    std::vector<StateImage> im((size_t)n_images);
-    for (int k = 0; k < n_images; k++)
-        if (parse_image(c, k, images[k], n_bytes[k], im[k])) return -1;
+    std::vector<MergeIn> in((size_t)n_images);
+    std::vector<const uint8_t*> stats((size_t)n_images);
+    const int64_t cw = c->counter_words;
+    int64_t words = 0;                        // the images' Stats and counter sections
+    for (int k = 0; k < n_images; k++) {
+        if (parse_image(c, k, images[k], n_bytes[k], in[k], stats[k])) return -1;
+        words += 2 * FPL_STATS_WORDS(in[k].src.rows) + cw;
+    }
     if (n_images == 0) return 0;
     CK(cudaSetDevice(c->device));
-    FplLists& L = c->lists;
-    const int64_t cw = c->counter_words;
-    int64_t rows = 0, used = c->used_cycles, reduced = c->reduced_rows, total[2] = {L.n[0], L.n[1]}, words = 0;
-    bool complete = L.complete, merged = L.merged;
-    for (const StateImage& s : im) {
-        rows = std::max(rows, s.rows);
-        used = std::max(used, s.used);
-        reduced = std::max(reduced, s.reduced);
-        complete = complete && s.complete;
-        merged = merged || s.merged;
-        for (int w = 0; w < 2; w++) total[w] += s.n[w];
-        words += 2 * FPL_STATS_WORDS(s.rows) + cw;
-    }
-    // the capacities first, as fpl_merge_stats grows them
-    if (reserve_cycles(c, rows)) return -1;
-    if (L.keep && (grow_list(c, 0, total[0]) || grow_list(c, 1, total[1]))) return -1;
-    CK(c->d_state_stage.grow(words));
-    CK(c->d_merge.grow(n_images));
-    std::vector<MergeSrc> tab((size_t)n_images);
-    int64_t at = 0;
-    for (int k = 0; k < n_images; k++) {
-        const int64_t sw = FPL_STATS_WORDS(im[k].rows);
-        unsigned long long* d = c->d_state_stage + at;
-        CK(cudaMemcpyAsync(d, im[k].stats, sizeof(unsigned long long) * (2 * sw + cw), cudaMemcpyHostToDevice, c->stream));
-        // the compact blocks as a source of capacity rows: k_merge_stats reads b * rows + c for c < rows, the tail at 16 * rows
-        tab[k] = MergeSrc{{d, d + sw}, d + 2 * sw, im[k].rows, im[k].rows};
-        at += 2 * sw + cw;
-    }
-    CK(cudaMemcpyAsync(c->d_merge, tab.data(), sizeof(MergeSrc) * n_images, cudaMemcpyHostToDevice, c->stream));
-    {
-        Timed t(c, K_MERGE_STATS);
-        launch_merge_stats(c->d_stats[0], c->d_stats[1], c->d_counters, c->C, rows, cw, c->d_merge, n_images, c->stream);
-    }
-    if (L.keep) {
-        for (int w = 0; w < 2; w++)
-            for (const StateImage& s : im) {
-                if (s.n[w])
-                    CK(cudaMemcpyAsync(L.d[w] + L.n[w], s.list[w], sizeof(HtmlEntry) * s.n[w], cudaMemcpyHostToDevice, c->stream));
-                L.n[w] += s.n[w];
-            }
-    } else {
-        complete = false;                     // the images' entries were not taken, as in a call with capture off
-    }
-    c->used_cycles = used; c->reduced_rows = reduced;
-    L.complete = complete; L.merged = merged;
-    c->rep.built = false; c->html.built = false;
-    CK(cudaGetLastError());
+    auto stage = [&] {
+        CK(c->d_state_stage.grow(words));
+        unsigned long long* d = c->d_state_stage;
+        for (int k = 0; k < n_images; k++) {
+            // the compact blocks as a source of capacity rows: k_merge_stats reads b * rows + c for c < rows, the tail at 16 * rows
+            const int64_t sw = FPL_STATS_WORDS(in[k].src.rows);
+            CK(cudaMemcpyAsync(d, stats[k], sizeof(unsigned long long) * (2 * sw + cw), cudaMemcpyHostToDevice, c->stream));
+            in[k].src.blk[0] = d; in[k].src.blk[1] = d + sw; in[k].src.cnt = d + 2 * sw;
+            d += 2 * sw + cw;
+        }
+        return 0;
+    };
+    if (merge_core(c, in, cudaMemcpyHostToDevice, stage)) return -1;
     CK(cudaStreamSynchronize(c->stream));
     collect_times(c);
     return 0;

@@ -259,7 +259,7 @@ k_emit_batch_copy(const EmitSource S, const int64_t* __restrict__ off, const Emi
 
 }  // namespace
 
-int fpl_emit_build(FplEmit* e, const EmitSource& src, bool want_failed, cudaStream_t s, char* err, size_t errlen) {
+int fpl_emit_build(FplEmit* e, const EmitSource& src, bool want_failed, cudaStream_t s, int& launched, char* err, size_t errlen) {
     e->built = false; e->out_bytes = e->failed_bytes = 0; e->with_failed = want_failed;
     const int64_t n = src.n_reads;
     if (n == 0) { e->built = true; return 0; }
@@ -269,6 +269,7 @@ int fpl_emit_build(FplEmit* e, const EmitSource& src, bool want_failed, cudaStre
     FPL_CK_ERR(cudaMemsetAsync(e->d_size + n, 0, sizeof(int64_t), s));
     FPL_CK_ERR(cudaMemsetAsync(e->d_size + 2 * n + 1, 0, sizeof(int64_t), s));
     k_emit_sizes<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src, want_failed, e->d_size);
+    launched++;
     FPL_CK_ERR(cub_call(e->d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, e->d_size.get(), e->d_off.get(), m, s); }));
     int64_t total_out = 0, total_both = 0;
     FPL_CK_ERR(cudaMemcpyAsync(&total_out, e->d_off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
@@ -281,6 +282,7 @@ int fpl_emit_build(FplEmit* e, const EmitSource& src, bool want_failed, cudaStre
     FPL_CK_ERR(e->d_failed.grow(e->failed_bytes + 16));
     const int64_t want = (n + 7) / 8;
     k_emit_copy<<<(unsigned)(want < FPL_NUM_SMS * 16 ? want : FPL_NUM_SMS * 16), 256, 0, s>>>(src, want_failed, e->d_off, e->d_out, e->d_failed);
+    launched++;
     FPL_CK_ERR(cudaGetLastError());
     e->built = true;
     return 0;
@@ -293,8 +295,9 @@ int fpl_emit_batch_reserve(FplBatchEmit* e, int64_t n_reads, char* err, size_t e
     return 0;
 }
 
-void launch_emit_batch_sizes(const EmitSource& src, int64_t* cnt, cudaStream_t s) {
+void launch_emit_batch_sizes(const EmitSource& src, int64_t* cnt, cudaStream_t s, int& launched) {
     k_emit_batch_sizes<<<(unsigned)((src.n_reads + 255) / 256), 256, 0, s>>>(src, cnt);
+    launched++;
 }
 
 int fpl_emit_batch_scan(FplBatchEmit* e, int64_t n_reads, cudaStream_t s, char* err, size_t errlen) {
@@ -308,7 +311,8 @@ int fpl_emit_batch_scan(FplBatchEmit* e, int64_t n_reads, cudaStream_t s, char* 
 }
 
 void launch_emit_batch_copy(const EmitSource& src, const int64_t* off, const EmitBatchOut& out, const EmitBatchOut& failed,
-                            cudaStream_t s) {
+                            cudaStream_t s, int& launched) {
     const int64_t want = (src.n_reads + 7) / 8;
     k_emit_batch_copy<<<(unsigned)(want < FPL_NUM_SMS * 16 ? want : FPL_NUM_SMS * 16), 256, 0, s>>>(src, off, out, failed);
+    launched++;
 }

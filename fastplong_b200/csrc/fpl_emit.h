@@ -48,11 +48,12 @@ struct EmitBatchOut {
     fpl_segment* segs;              // may be null
 };
 
-int fpl_emit_build(FplEmit* e, const EmitSource& src, bool want_failed, cudaStream_t s, char* err, size_t errlen);
+// launched += the kernels it enqueued, also when it then fails; so do launch_emit_batch_*
+int fpl_emit_build(FplEmit* e, const EmitSource& src, bool want_failed, cudaStream_t s, int& launched, char* err, size_t errlen);
 
 // fpl_emit_batch_device: reserve -> launch_emit_batch_sizes -> scan (synchronous: the totals come to the host) -> copy
 int fpl_emit_batch_reserve(FplBatchEmit* e, int64_t n_reads, char* err, size_t errlen);
-void launch_emit_batch_sizes(const EmitSource& src, int64_t* cnt, cudaStream_t s);
+void launch_emit_batch_sizes(const EmitSource& src, int64_t* cnt, cudaStream_t s, int& launched);
 int fpl_emit_batch_scan(FplBatchEmit* e, int64_t n_reads, cudaStream_t s, char* err, size_t errlen);
 void launch_emit_batch_copy(const EmitSource& src, const int64_t* off, const EmitBatchOut& out, const EmitBatchOut& failed,
-                            cudaStream_t s);
+                            cudaStream_t s, int& launched);

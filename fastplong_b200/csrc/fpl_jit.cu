@@ -98,7 +98,7 @@ std::string gen_counter(int which, const char* adapter) {
 }
 
 std::string scan_source_v2(const char* a0, const char* a1) {
-    std::string src = kScanJit2Source;
+    std::string src = "#define QH_STRIPES " + std::to_string(QH_STRIPES) + "\n" + kScanJit2Source;
     const std::string marker = "//@@COUNTERS@@";
     const size_t at = src.find(marker);
     src.replace(at, marker.size(), gen_counter(0, a0) + gen_counter(1, a1));
@@ -177,7 +177,7 @@ int fpl_jit_build_scan(int device, const char* a0, const char* a1, bool doAdapte
     return 0;
 }
 
-int fpl_jit_launch_scan(const FplJitKernel* k, const DevBatch& b, ReadState* st, cudaStream_t stream) {
+int fpl_jit_launch_scan(const FplJitKernel* k, const DevBatch& b, ReadState* st, cudaStream_t stream, int& launched) {
     if (b.n_reads == 0) return 0;
     const uint8_t* seq = b.seq;
     const uint8_t* qual = b.qual;
@@ -190,5 +190,7 @@ int fpl_jit_launch_scan(const FplJitKernel* k, const DevBatch& b, ReadState* st,
     // one CTA per read: the hardware scheduler balances the gamma-distributed read lengths better than persistent CTAs
     // walking the reads round-robin.
     CUresult cr = driver().LaunchKernel((CUfunction)k->fn, (unsigned)b.n_reads, 1, 1, 128, 1, 1, 0, (CUstream)stream, args, nullptr);
-    return cr == CUDA_SUCCESS ? 0 : -1;
+    if (cr != CUDA_SUCCESS) return -1;
+    launched++;
+    return 0;
 }

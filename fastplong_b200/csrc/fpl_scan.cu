@@ -8,6 +8,7 @@
 // positions at a time (SWAR on 32-bit words).  k_final then verifies the arg-mins with one edit distance each,
 // derives the segments (Read::breakByGap, src/read.cpp:192-215) and evaluates the filter thresholds.
 #include "fpl_device.cuh"
+#include "fpl_scan.h"
 
 #define SCAN_THREADS 256
 #define SCAN_TILE 4096                      // positions per tile (multiple of 4*SCAN_THREADS... see loop)
@@ -151,9 +152,10 @@ k_scan(const __grid_constant__ DevParams P, DevBatch b, ReadState* __restrict__ 
     }
 }
 
-void launch_scan(const DevParams& P, const DevBatch& b, ReadState* st, cudaStream_t stream) {
+void launch_scan(const DevParams& P, const DevBatch& b, ReadState* st, cudaStream_t stream, int& launched) {
     if (b.n_reads == 0) return;
     k_scan<<<(unsigned)b.n_reads, SCAN_THREADS, 0, stream>>>(P, b, st);
+    launched++;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -437,7 +439,7 @@ k_final(const __grid_constant__ DevParams P, DevBatch b, const ReadState* __rest
 
 // exc / n_exc (nullptr: k_scan_jit did not count the quality histograms): the list of the reads k_read_qual_exc treats
 void launch_final(const DevParams& P, const DevBatch& b, const ReadState* st, fpl_read_result* res, StatSeg* postseg,
-                  int32_t* exc, int* n_exc, cudaStream_t stream) {
+                  int32_t* exc, int* n_exc, cudaStream_t stream, int& launched) {
     if (b.n_reads == 0) return;
     unsigned grid = (unsigned)((b.n_reads + FINAL_WARPS - 1) / FINAL_WARPS);
     if (exc) {
@@ -447,6 +449,7 @@ void launch_final(const DevParams& P, const DevBatch& b, const ReadState* st, fp
         if (P.small_adapters == 0) k_final<0, false><<<grid, FINAL_WARPS * 32, 0, stream>>>(P, b, st, res, postseg, exc, n_exc);
         else k_final<2, false><<<grid, FINAL_WARPS * 32, 0, stream>>>(P, b, st, res, postseg, exc, n_exc);
     }
+    launched++;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -521,7 +524,8 @@ k_count(const fpl_read_result* __restrict__ res, int64_t n, unsigned long long* 
 // count_segments = false: --mask/--break, where the output reads are counted by k_ext_filter instead.  stats_pre /
 // stats_post / C (stats_pre == nullptr: not here): see k_count.
 void launch_count(const fpl_read_result* res, int64_t n, unsigned long long* counters, bool count_segments, const int32_t* lens,
-                  unsigned long long* stats_pre, unsigned long long* stats_post, int64_t C, cudaStream_t stream) {
+                  unsigned long long* stats_pre, unsigned long long* stats_post, int64_t C, cudaStream_t stream, int& launched) {
     if (n == 0) return;
     k_count<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(res, n, counters, count_segments, lens, stats_pre, stats_post, C);
+    launched++;
 }

@@ -18,6 +18,7 @@
 // the complexity count compares each word with itself shifted by one byte.
 #include "fpl_device.cuh"
 #include "fpl_scanplan.h"
+#include "fpl_scan.h"
 
 #define SF_WARPS 4
 #define SF_THREADS (SF_WARPS * 32)
@@ -308,7 +309,7 @@ k_scan_fast(const __grid_constant__ DevParams P, const __grid_constant__ ScanPla
     }
 }
 
-void launch_scan_fast(const DevParams& P, const ScanPlan& plan, const DevBatch& b, ReadState* st, cudaStream_t stream) {
+void launch_scan_fast(const DevParams& P, const ScanPlan& plan, const DevBatch& b, ReadState* st, cudaStream_t stream, int& launched) {
     if (b.n_reads == 0) return;
     const unsigned grid = (unsigned)b.n_reads;
 #define SF_LAUNCH(N, H) k_scan_fast<N, H><<<grid, SF_THREADS, 0, stream>>>(P, plan, b, st)
@@ -323,4 +324,5 @@ void launch_scan_fast(const DevParams& P, const ScanPlan& plan, const DevBatch& 
         default: SF_LAUNCH(8, 4); break;
     }
 #undef SF_LAUNCH
+    launched++;
 }

@@ -640,11 +640,11 @@ __global__ void k_cs_gather(const StatSeg* __restrict__ segs, const uint32_t* __
 // them.  fused_post (with do_kmer, segs = the pre-filter list, one per read): the post-filter list; the segments
 // cs_fused_takes accepts are counted into stats_post by the same pass.  residual_of (segs = that post-filter list): the
 // pre-filter list of the fused pass, whose segments this pass skips.  Returns 0, or -1 when the workspace cannot be
-// allocated.
+// allocated (before any launch).
 int launch_cycle_stats(CycleWs* ws, const uint8_t* seq, const uint8_t* qual, const StatSeg* segs, int64_t nseg, int64_t max_len,
                        unsigned long long* stats, int64_t C, bool do_kmer, unsigned long long* kmer_also, bool aligned,
                        const StatSeg* fused_post, unsigned long long* stats_post, const StatSeg* residual_of,
-                       cudaStream_t stream) {
+                       cudaStream_t stream, int& launched) {
     if (nseg == 0 || max_len <= 0) return 0;
     // the opt-in to more than 48 KB of dynamic shared memory is a per-device function attribute
     static std::atomic<unsigned long long> attr_set{0};
@@ -700,6 +700,7 @@ int launch_cycle_stats(CycleWs* ws, const uint8_t* seq, const uint8_t* qual, con
         else if (do_kmer) k_cycle_stats<true, CS_NT_KMER, CS_DEPTH_KMER, false, false><<<grid, CS_NT_KMER, CS_SMEM_KMER, stream>>>(seq, qual, sorted, nseg, stats, C, kmer_also, nullptr, 1u, al);
         else k_cycle_stats<false, CS_NT_PLAIN, CS_DEPTH_PLAIN, false, false><<<grid, CS_NT_PLAIN, CS_SMEM_PLAIN, stream>>>(seq, qual, sorted, nseg, stats, C, nullptr, nullptr, 1u, al);
     }
+    launched += 3;                       // k_cs_keys, k_cs_gather (around the library's radix sort), k_cycle_stats
     return 0;
 }
 
@@ -801,11 +802,12 @@ k_kmer_fix(DevBatch b, const fpl_read_result* __restrict__ res, unsigned long lo
         if (rem[i]) atomicAdd(&post_kmer[i], 0ull - (unsigned long long)rem[i]);
 }
 
-void launch_kmer_fix(const DevBatch& b, const fpl_read_result* res, unsigned long long* post_kmer, cudaStream_t stream) {
+void launch_kmer_fix(const DevBatch& b, const fpl_read_result* res, unsigned long long* post_kmer, cudaStream_t stream, int& launched) {
     if (b.n_reads == 0) return;
     const int64_t want = (b.n_reads + KF_WARPS - 1) / KF_WARPS;
     const unsigned grid = (unsigned)(want < FPL_NUM_SMS * 16 ? want : FPL_NUM_SMS * 16);
     k_kmer_fix<<<grid, KF_WARPS * 32, 0, stream>>>(b, res, post_kmer);
+    launched++;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1000,12 +1002,13 @@ k_read_qual(DevBatch b, unsigned long long* __restrict__ stats_pre, unsigned lon
 }
 
 void launch_read_qual(const DevBatch& b, unsigned long long* stats_pre, unsigned long long* stats_post, int64_t C,
-                      fpl_read_result* res, bool pre_only, cudaStream_t stream) {
+                      fpl_read_result* res, bool pre_only, cudaStream_t stream, int& launched) {
     if (b.n_reads == 0) return;
     // persistent-ish grid: enough blocks to fill the GPU several times over, each warp strides over the reads
     const int64_t want = (b.n_reads + RQ_WARPS - 1) / RQ_WARPS;
     const unsigned grid = (unsigned)(want < FPL_NUM_SMS * 64 ? want : FPL_NUM_SMS * 64);
     k_read_qual<<<grid, RQ_WARPS * 32, 0, stream>>>(b, stats_pre, stats_post, C, res, pre_only);
+    launched++;
 }
 
 // k_read_qual's work for the reads k_final listed (exc[0, *n_exc)) when k_scan_jit counted the quality histograms: the
@@ -1052,12 +1055,13 @@ k_read_qual_exc(DevBatch b, const ReadState* __restrict__ st, const int32_t* __r
 }
 
 void launch_read_qual_exc(const DevBatch& b, const ReadState* st, const int32_t* exc, const int* n_exc, unsigned long long* stats_pre,
-                          unsigned long long* stats_post, int64_t C, fpl_read_result* res, cudaStream_t stream) {
+                          unsigned long long* stats_post, int64_t C, fpl_read_result* res, cudaStream_t stream, int& launched) {
     if (b.n_reads == 0) return;
     // the list is a few percent of the reads: a grid of a few blocks per SM, capped by what the whole batch would need
     const int64_t want = (b.n_reads + RQ_WARPS - 1) / RQ_WARPS;
     const unsigned grid = (unsigned)(want < FPL_NUM_SMS * 8 ? want : FPL_NUM_SMS * 8);
     k_read_qual_exc<<<grid, RQ_WARPS * 32, 0, stream>>>(b, st, exc, n_exc, stats_pre, stats_post, C, res);
+    launched++;
 }
 
 // the striped sums of k_scan_jit's histograms ([QH_STRIPES][2][128]: whole reads, windows) -> mBaseQualHistogram of the
@@ -1071,8 +1075,9 @@ __global__ void k_qhist_fold(const unsigned long long* __restrict__ stripes, int
 }
 
 void launch_qhist_fold(const unsigned long long* stripes, int n_stripes, unsigned long long* stats_pre, unsigned long long* stats_post,
-                       int64_t C, cudaStream_t stream) {
+                       int64_t C, cudaStream_t stream, int& launched) {
     k_qhist_fold<<<1, 256, 0, stream>>>(stripes, n_stripes, stats_pre, stats_post, C);
+    launched++;
 }
 
 // pre-stats segment list: every input read, full length
@@ -1084,9 +1089,10 @@ __global__ void k_make_preseg(DevBatch b, StatSeg* __restrict__ segs) {
     segs[r] = s;
 }
 
-void launch_make_preseg(const DevBatch& b, StatSeg* segs, cudaStream_t stream) {
+void launch_make_preseg(const DevBatch& b, StatSeg* segs, cudaStream_t stream, int& launched) {
     if (b.n_reads == 0) return;
     k_make_preseg<<<(unsigned)((b.n_reads + 255) / 256), 256, 0, stream>>>(b, segs);
+    launched++;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1254,21 +1260,24 @@ __global__ void k_report_frame(const uint8_t* __restrict__ frame, const int64_t*
 }  // namespace
 
 void launch_report_cycles(const unsigned long long* pre, const unsigned long long* post, int64_t C, unsigned long long* sum,
-                          cudaStream_t stream) {
+                          cudaStream_t stream, int& launched) {
     const int64_t want = (C + 255) / 256;
     k_report_cycles<<<dim3((unsigned)(want < FPL_NUM_SMS * 8 ? want : FPL_NUM_SMS * 8), 2), 256, 0, stream>>>(pre, post, C, sum);
+    launched++;
 }
 
-void launch_report_sizes(const ReportCurves& R, int64_t* size, cudaStream_t stream) {
+void launch_report_sizes(const ReportCurves& R, int64_t* size, cudaStream_t stream, int& launched) {
     const int64_t n = R.T[0] + R.T[1];
     if (n) k_report_sizes<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(R, size);
+    launched += n != 0;
 }
 
 void launch_report_text(const ReportCurves& R, const int64_t* off, const uint8_t* frame, const int64_t* src, const int64_t* dst,
-                        int n_pieces, uint8_t* text, cudaStream_t stream) {
+                        int n_pieces, uint8_t* text, cudaStream_t stream, int& launched) {
     k_report_frame<<<n_pieces, 256, 0, stream>>>(frame, src, dst, text);
     const int64_t n = R.T[0] + R.T[1];
     if (n) k_report_text<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(R, off, text);
+    launched += n ? 2 : 1;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1470,54 +1479,65 @@ unsigned grid_for(int64_t n, int64_t cap) {
 }  // namespace
 
 void launch_html_capture(const fpl_read_result* res, const int32_t* lens, int64_t n, const fpl_segment* segs, int64_t n_segs,
-                         HtmlEntry* pre, HtmlEntry* post, cudaStream_t stream) {
+                         HtmlEntry* pre, HtmlEntry* post, cudaStream_t stream, int& launched) {
     const int64_t m = n > n_segs ? n : n_segs;
     if (m) k_html_capture<<<grid_for(m, FPL_NUM_SMS * 8), 256, 0, stream>>>(res, lens, n, segs, n_segs, pre, post);
+    launched += m != 0;
 }
 
-void launch_html_hist(const HtmlEntry* e, int64_t n, int64_t nchunks, long long* mat, cudaStream_t stream) {
+void launch_html_hist(const HtmlEntry* e, int64_t n, int64_t nchunks, long long* mat, cudaStream_t stream, int& launched) {
     if (nchunks) k_html_hist<<<(unsigned)((nchunks + 3) / 4), 128, 0, stream>>>(e, n, nchunks, mat);
+    launched += nchunks != 0;
 }
 
-void launch_html_scatter(const HtmlEntry* e, int64_t n, int64_t nchunks, const long long* off, HtmlEntry* out, cudaStream_t stream) {
+void launch_html_scatter(const HtmlEntry* e, int64_t n, int64_t nchunks, const long long* off, HtmlEntry* out, cudaStream_t stream, int& launched) {
     if (nchunks) k_html_scatter<<<(unsigned)((nchunks + 3) / 4), 128, 0, stream>>>(e, n, nchunks, off, out);
+    launched += nchunks != 0;
 }
 
-void launch_html_lenhist(const HtmlEntry* e, int64_t n, unsigned long long* hist, cudaStream_t stream) {
+void launch_html_lenhist(const HtmlEntry* e, int64_t n, unsigned long long* hist, cudaStream_t stream, int& launched) {
     if (n) k_html_lenhist<<<grid_for(n, FPL_NUM_SMS * 8), 256, 0, stream>>>(e, n, hist);
+    launched += n != 0;
 }
 
-void launch_html_lenprod(const unsigned long long* cnt, int64_t H, long long* prod, cudaStream_t stream) {
+void launch_html_lenprod(const unsigned long long* cnt, int64_t H, long long* prod, cudaStream_t stream, int& launched) {
     k_html_lenprod<<<(unsigned)((H + 255) / 256), 256, 0, stream>>>(cnt, H, prod);
+    launched++;
 }
 
 void launch_html_lensearch(const unsigned long long* cnt, const long long* ccum, const long long* prod, const long long* pcum,
-                           int64_t H, long long half_sum, unsigned long long half_n, int* out, cudaStream_t stream) {
+                           int64_t H, long long half_sum, unsigned long long half_n, int* out, cudaStream_t stream, int& launched) {
     k_html_lensearch<<<(unsigned)((H + 255) / 256), 256, 0, stream>>>(cnt, ccum, prod, pcum, H, half_sum, half_n, out);
+    launched++;
 }
 
-void launch_html_bins(const unsigned long long* blk, int64_t C, int64_t T, unsigned long long* out, cudaStream_t stream) {
+void launch_html_bins(const unsigned long long* blk, int64_t C, int64_t T, unsigned long long* out, cudaStream_t stream, int& launched) {
     if (T) k_html_bins<<<grid_for(T, FPL_NUM_SMS * 8), 256, 0, stream>>>(blk, C, T, out);
+    launched += T != 0;
 }
 
-void launch_html_values(const unsigned long long* blk, int64_t C, int64_t T, int is_rna, double* vals, cudaStream_t stream) {
+void launch_html_values(const unsigned long long* blk, int64_t C, int64_t T, int is_rna, double* vals, cudaStream_t stream, int& launched) {
     if (T) k_html_values<<<grid_for(11 * T, FPL_NUM_SMS * 16), 256, 0, stream>>>(blk, C, T, is_rna, vals);
+    launched += T != 0;
 }
 
-void launch_html_sums(const double* vals, int64_t T, const long long* x, int64_t R, double* sums, cudaStream_t stream) {
+void launch_html_sums(const double* vals, int64_t T, const long long* x, int64_t R, double* sums, cudaStream_t stream, int& launched) {
     if (R) k_html_sums<<<(unsigned)((11 * R + 127) / 128), 128, 0, stream>>>(vals, T, x, R, sums);
+    launched += R != 0;
 }
 
-void launch_html_sizes(const HtmlText& H, int64_t* size, cudaStream_t stream) {
+void launch_html_sizes(const HtmlText& H, int64_t* size, cudaStream_t stream, int& launched) {
     const int64_t n = H.start[HTML_SEGS];
     if (n) k_html_sizes<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(H, size);
+    launched += n != 0;
 }
 
 void launch_html_text(const HtmlText& H, const int64_t* off, const uint8_t* frame, const int64_t* src, const int64_t* dst, int n_pieces,
-                      uint8_t* text, cudaStream_t stream) {
+                      uint8_t* text, cudaStream_t stream, int& launched) {
     k_report_frame<<<n_pieces, 256, 0, stream>>>(frame, src, dst, text);
     const int64_t n = H.start[HTML_SEGS];
     if (n) k_html_text<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(H, off, text);
+    launched += n ? 2 : 1;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1560,7 +1580,8 @@ __global__ void k_merge_stats(unsigned long long* __restrict__ pre, unsigned lon
 }  // namespace
 
 void launch_merge_stats(unsigned long long* pre, unsigned long long* post, unsigned long long* cnt, int64_t C, int64_t rows,
-                        int64_t cnt_words, const MergeSrc* src, int n_src, cudaStream_t stream) {
+                        int64_t cnt_words, const MergeSrc* src, int n_src, cudaStream_t stream, int& launched) {
     const int64_t total = 2 * (16 * rows + FPL_STATS_TAIL) + cnt_words;
     k_merge_stats<<<grid_for(total, FPL_NUM_SMS * 8), 256, 0, stream>>>(pre, post, cnt, C, rows, cnt_words, src, n_src);
+    launched++;
 }

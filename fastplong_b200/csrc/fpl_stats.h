@@ -1,9 +1,12 @@
-// Workspace of launch_cycle_stats (the length-sorted segment list), owned by a context: one stream, one workspace.
+// fpl_stats.cu's launchers, each adding the kernels it enqueues to its last argument, and the descriptors they take.
 #pragma once
 #include <cstddef>
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "fpl_buf.h"
+#include "fpl_device.cuh"
+
+// Workspace of launch_cycle_stats (the length-sorted segment list), owned by a context: one stream, one workspace.
 
 struct SegD;
 struct CycleWs {
@@ -33,7 +36,7 @@ struct MergeSrc {
 // k_merge_stats: rows [0, rows) and the tail of dst's two blocks (capacity C), and its cnt_words counters, += each of the n_src
 // sources' (a device table), in table order; one launch
 void launch_merge_stats(unsigned long long* pre, unsigned long long* post, unsigned long long* cnt, int64_t C, int64_t rows,
-                        int64_t cnt_words, const MergeSrc* src, int n_src, cudaStream_t stream);
+                        int64_t cnt_words, const MergeSrc* src, int n_src, cudaStream_t stream, int& launched);
 
 // fpl_keep_read_lists: one entry per read of a Stats block, in the order Stats::statRead saw them.  A post-filter slot that
 // holds no output read (a failing or missing segment) has len = -1; the report drops it.
@@ -59,3 +62,29 @@ struct HtmlText {
     const double* sums[2];              // curve values
     const long long* x[2];              // each block's x list: range i is [x[i - 1], x[i]), x[-1] = 0
 };
+
+int launch_cycle_stats(CycleWs*, const uint8_t*, const uint8_t*, const StatSeg*, int64_t, int64_t, unsigned long long*, int64_t,
+                       bool, unsigned long long*, bool, const StatSeg*, unsigned long long*, const StatSeg*, cudaStream_t, int&);
+void launch_kmer_fix(const DevBatch&, const fpl_read_result*, unsigned long long*, cudaStream_t, int&);
+void launch_read_qual(const DevBatch&, unsigned long long*, unsigned long long*, int64_t, fpl_read_result*, bool, cudaStream_t, int&);
+void launch_read_qual_exc(const DevBatch&, const ReadState*, const int32_t*, const int*, unsigned long long*, unsigned long long*, int64_t,
+                          fpl_read_result*, cudaStream_t, int&);
+void launch_qhist_fold(const unsigned long long*, int, unsigned long long*, unsigned long long*, int64_t, cudaStream_t, int&);
+void launch_make_preseg(const DevBatch&, StatSeg*, cudaStream_t, int&);
+void launch_report_cycles(const unsigned long long*, const unsigned long long*, int64_t, unsigned long long*, cudaStream_t, int&);
+void launch_report_sizes(const ReportCurves&, int64_t*, cudaStream_t, int&);
+void launch_report_text(const ReportCurves&, const int64_t*, const uint8_t*, const int64_t*, const int64_t*, int, uint8_t*, cudaStream_t,
+                        int&);
+void launch_html_capture(const fpl_read_result*, const int32_t*, int64_t, const fpl_segment*, int64_t, HtmlEntry*, HtmlEntry*, cudaStream_t,
+                         int&);
+void launch_html_hist(const HtmlEntry*, int64_t, int64_t, long long*, cudaStream_t, int&);
+void launch_html_scatter(const HtmlEntry*, int64_t, int64_t, const long long*, HtmlEntry*, cudaStream_t, int&);
+void launch_html_lenhist(const HtmlEntry*, int64_t, unsigned long long*, cudaStream_t, int&);
+void launch_html_lenprod(const unsigned long long*, int64_t, long long*, cudaStream_t, int&);
+void launch_html_lensearch(const unsigned long long*, const long long*, const long long*, const long long*, int64_t, long long,
+                           unsigned long long, int*, cudaStream_t, int&);
+void launch_html_bins(const unsigned long long*, int64_t, int64_t, unsigned long long*, cudaStream_t, int&);
+void launch_html_values(const unsigned long long*, int64_t, int64_t, int, double*, cudaStream_t, int&);
+void launch_html_sums(const double*, int64_t, const long long*, int64_t, double*, cudaStream_t, int&);
+void launch_html_sizes(const HtmlText&, int64_t*, cudaStream_t, int&);
+void launch_html_text(const HtmlText&, const int64_t*, const uint8_t*, const int64_t*, const int64_t*, int, uint8_t*, cudaStream_t, int&);

@@ -6,6 +6,7 @@
 // candidate positions at once, a ballot / min-reduction picks what the sequential loop would have picked.
 // Work is O(window) per read, not O(read length), except for degenerate quality cuts.
 #include "fpl_device.cuh"
+#include "fpl_scan.h"
 
 namespace {
 
@@ -726,7 +727,7 @@ k_trim_fasta(const __grid_constant__ DevParams P, DevBatch b, ReadState* __restr
 }
 
 void launch_trim(const DevParams& P, const DevBatch& b, ReadState* st, fpl_read_result* res,
-                 unsigned long long* counters, cudaStream_t stream) {
+                 unsigned long long* counters, cudaStream_t stream, int& launched) {
     if (b.n_reads == 0) return;
     unsigned grid = (unsigned)((b.n_reads + TRIM_WARPS - 1) / TRIM_WARPS);
     if (P.small_adapters == 0) k_trim<0><<<grid, TRIM_WARPS * 32, 0, stream>>>(P, b, st, res, counters);
@@ -737,4 +738,5 @@ void launch_trim(const DevParams& P, const DevBatch& b, ReadState* st, fpl_read_
         else if (P.fasta_class == 1) k_trim_fasta<1><<<grid, TRIM_WARPS * 32, 0, stream>>>(P, b, st, res, counters);
         else k_trim_fasta<2><<<grid, TRIM_WARPS * 32, 0, stream>>>(P, b, st, res, counters);
     }
+    launched += P.opt.adapter_enabled && P.n_adapters > 2 ? 2 : 1;
 }

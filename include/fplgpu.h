@@ -575,6 +575,8 @@ int fpl_reset(fpl_ctx* ctx);
  * stream and zeroes the per-kernel totals; fpl_last_kernel_times returns, per kernel, the device time (ms) and
  * the number of timed launches accumulated since then (call after fpl_sync).  names/ms/launches hold up to cap
  * entries; returns the number of kernels.  fpl_launch_count = kernel launches made by the context so far.
+ * It counts the library's own kernels, but not the read-length reduction of fpl_process_device, the --mask/--break
+ * stage's kernels, the FASTQ ingest's kernels, or the kernels of cub and NCCL.
  */
 int fpl_last_kernel_times(fpl_ctx* ctx, const char** names, float* ms, int64_t* launches, int cap);
 int64_t fpl_launch_count(fpl_ctx* ctx);

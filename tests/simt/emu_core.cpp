@@ -46,6 +46,23 @@ extern "C" long long emu_live_allocs() { return emu::live_allocs; }
 // -> the count it replaces: > 0 when the allocation it was set for never came
 extern "C" long long emu_fail_alloc(long long k) { const long long was = emu::fail_alloc_in; emu::fail_alloc_in = k; return was; }
 extern "C" long long emu_blocks() { return (long long)emu::block_serial; }
+// kernel name ("k_trim" of "k_trim<1>(P, b, ...)", "k_scan_jit" of "jit::k_scan_jit(...)") -> launches so far
+namespace emu { namespace { std::mutex launch_count_mu; std::map<std::string, long long> launch_count; } }
+void emu::note_launch(const char* call) {
+    std::string name(call);
+    name = name.substr(0, name.find_first_of("<( "));
+    if (name.rfind("::") != std::string::npos) name = name.substr(name.rfind("::") + 2);
+    std::lock_guard<std::mutex> lock(launch_count_mu);
+    launch_count[name]++;
+}
+// -> the launches so far of the kernels whose names start with prefix ("": all)
+extern "C" long long emu_launches(const char* prefix) {
+    std::lock_guard<std::mutex> lock(emu::launch_count_mu);
+    long long n = 0;
+    for (const auto& kv : emu::launch_count)
+        if (kv.first.compare(0, strlen(prefix), prefix) == 0) n += kv.second;
+    return n;
+}
 
 // ---------------- streams and events (fake/cuda_runtime.h): ids never reused; the live ones, an event with its timestamp ----------------
 namespace emu {

@@ -63,6 +63,7 @@ int tid_in_block();
 // deposit v, wait for the group, return the group's generation result (res[], res_mask valid until the next collective)
 Group& collect(Group& g, int index, uint64_t v);
 void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body);
+void note_launch(const char* call);     // counts a launch under its kernel's name (emu_core.cpp: emu_launches)
 extern long long collectives;
 extern unsigned long long block_serial;      // counts the blocks run so far (per-thread emulation state resets on a new block)
 extern uint8_t* dynamic_smem;          // `extern __shared__` of the running kernel
@@ -165,4 +166,5 @@ template <class T, class U> static inline T atomicExch(T* p, U v) { T o = *p; *p
 template <class T, class U, class V> static inline T atomicCAS(T* p, U cmp, V v) { T o = *p; if (o == (T)cmp) *p = (T)v; return o; }
 
 // KERNEL<<<grid, block, smem, stream>>>(args) is rewritten by tests/simt_emu.py into EMU_LAUNCH(grid, block, smem, KERNEL(args))
-#define EMU_LAUNCH(grid, block, smem, ...) emu::launch(dim3(grid), dim3(block), (size_t)(smem), [&]() { __VA_ARGS__; })
+#define EMU_LAUNCH(grid, block, smem, ...) \
+    (emu::note_launch(#__VA_ARGS__), emu::launch(dim3(grid), dim3(block), (size_t)(smem), [&]() { __VA_ARGS__; }))

@@ -79,8 +79,8 @@ def _rewrite_launches(text):
 
 
 # ---- the build ----
-LIB_SOURCES = ("fpl_api.cu", "fpl_trim.cu", "fpl_scan.cu", "fpl_scan_fast.cu", "fpl_stats.cu", "fpl_jit.cu", "fpl_ingest.cu", "fpl_ext.cu",
-               "fpl_eval.cu", "fpl_emit.cu")
+# the library's translation units: csrc/Makefile's SRC
+LIB_SOURCES = tuple(re.search(r"^SRC := (.*)$", open(os.path.join(CSRC, "Makefile")).read(), re.M).group(1).split())
 
 
 def _lib_text(fn, text=None):
@@ -189,11 +189,14 @@ def emulated_library():
     cudaMalloc / cudaMallocHost blocks not yet freed; emu_fail_alloc(k): the k-th allocation from now fails, once, 0 = none; it
     returns the count it replaces, > 0 when that allocation never came.  emu_live_handles, emu_fail_handle(k): the same for stream
     and event creations, where a failed one writes a poison handle; emu_failed_handle_kind(): what that creation was (EMU_STREAM,
-    EMU_EVENT, EMU_TIMING_EVENT, 0: none), then 0; emu_bad_handles: calls that got a handle that was not live)"""
+    EMU_EVENT, EMU_TIMING_EVENT, 0: none), then 0; emu_bad_handles: calls that got a handle that was not live; emu_launches(prefix):
+    the kernel launches so far whose kernel names start with prefix, b"" for all)"""
     lib = C.CDLL(build_library())
     lib.emu_set_cp_async_lazy.argtypes = [C.c_int]
     lib.emu_collectives.restype = lib.emu_blocks.restype = lib.emu_live_allocs.restype = C.c_longlong
     lib.emu_live_handles.restype = lib.emu_bad_handles.restype = lib.emu_failed_handle_kind.restype = C.c_longlong
+    lib.emu_launches.argtypes = [C.c_char_p]
+    lib.emu_launches.restype = C.c_longlong
     for f in (lib.emu_fail_alloc, lib.emu_fail_handle):
         f.argtypes = [C.c_longlong]
         f.restype = C.c_longlong

@@ -4,7 +4,9 @@ stream and event creations do the same (emu_live_handles, emu_fail_handle) and c
 (emu_bad_handles).  A context frees everything its entry points allocated or created when it is destroyed; an allocation that fails
 anywhere in a call makes the call fail and leaks nothing; so does a stream or event creation, except a timing event, whose launch
 then runs untimed; fpl_stats_reserve is all or nothing; a report or emit build that failed gives the same bytes when it is called
-again."""
+again.  Whether a call succeeds or fails, fpl_launch_count goes up by the kernels it ran, as the emulator counts them
+(emu_launches)."""
+import dataclasses
 import gc
 
 import numpy as np
@@ -13,12 +15,18 @@ import pytest
 import cases
 import layouts
 import simt_emu
-from fastplong_b200 import abi, synth
+from fastplong_b200 import abi, pack, synth
 from fastplong_b200.binding import FplError
 
 PLAIN, EXT = cases.OPTION_SETS["cut_polyx_cplx"], cases.MASK_BREAK_SETS["mask_and_break"]
 BATCH = cases.blocky_quality_batch(5, n=12)
 TEXT = b"".join(b"@r%d\n%s\n+\n%s\n" % (i, *BATCH.read(i)) for i in range(BATCH.n_reads))
+EMPTY = pack.PackedBatch(*(np.zeros(pack.TAIL_PAD, np.uint8) for _ in range(2)), np.zeros(3, np.int64), np.zeros(3, np.int32))
+# every base Q2: with --mask/--break no output read is left, so no post-filter segment
+VANISH = dataclasses.replace(BATCH, qual=np.full_like(BATCH.qual, ord("#")))
+# kernels outside fpl_launch_count: fpl_process_device's length reduction, the --mask/--break stage, the FASTQ ingest, and
+# fpl_eval_adapter_kmers (no context's); cub's and NCCL's kernels are not emulator launches
+UNCOUNTED = (b"k_lens_minmax", b"k_ext_", b"k_count_lines", b"k_fastq_", b"k_eval_")
 
 
 @pytest.fixture(scope="module")
@@ -51,6 +59,26 @@ def with_source(e):
     e.src.process(BATCH)
 
 
+def with_image(e):
+    """e has processed a batch, e.image is the state of another context that has: fpl_state_merge(e, [e.image]) is ready"""
+    e.process(BATCH)
+    src = engine(e.options)
+    src.process(BATCH)
+    e.image = src.export_state()
+    src.close()
+
+
+def counted(lib, e, call):
+    """call(e), which may raise; either way fpl_launch_count has gone up by the counted kernels the emulator ran"""
+    def ran():
+        return lib.emu_launches(b"") - sum(lib.emu_launches(p) for p in UNCOUNTED)
+    before = e.launch_count, ran()
+    try:
+        return call(e)
+    finally:
+        assert e.launch_count - before[0] == ran() - before[1], "fpl_launch_count against the kernels run"
+
+
 def close(e):
     for x in (e, getattr(e, "src", None)):
         if x:
@@ -68,6 +96,10 @@ ENTRIES = {
     "fpl_report_html": (lambda e: e.process(BATCH), lambda e: e.report_html(command="fastplong -i x", time_text="t"), True),
     "fpl_merge_stats": (with_source, lambda e: e.merge(e.src), False),
     "fpl_stats_reserve": (lambda e: e.process(BATCH), lambda e: e.reserve_cycles(1 << 14), False),
+    "fpl_state_merge": (with_image, lambda e: e.merge_state(e.image), False),
+    "fpl_process_host of empty reads": (None, lambda e: e.process(EMPTY), False),
+    "fpl_process_host of reads without output": (None, lambda e: e.process(VANISH), False),
+    "fpl_report_json on a fresh context": (lambda e: None, lambda e: e.report_json(command="fastplong -i x"), True),
 }
 
 
@@ -139,7 +171,7 @@ def test_an_allocation_failure_leaks_nothing(lib, opt, entry):
             before(e)
         lib.emu_fail_alloc(k)
         try:
-            call(e)
+            counted(lib, e, call)
             failed = False
         except FplError:
             failed = True
@@ -149,7 +181,7 @@ def test_an_allocation_failure_leaks_nothing(lib, opt, entry):
         else:
             assert failed, f"{entry}: allocation {k} failed, the call succeeded"
             if retry:
-                assert call(e) == want, f"{entry} retried after allocation {k} failed"
+                assert counted(lib, e, call) == want, f"{entry} retried after allocation {k} failed"
         close(e)
         assert live(lib) == base, f"{entry}: allocation {k} failed: leak"
         if pending:
@@ -201,7 +233,7 @@ def test_every_entry_point_releases_its_streams_events_and_blocks(lib, monkeypat
         e.set_timing(timing)
         if before:
             before(e)
-        call(e)
+        counted(lib, e, call)
         close(e)
         assert held(lib) == base, entry
 
@@ -245,7 +277,7 @@ def test_a_failed_stream_or_event_creation_leaks_nothing(lib, monkeypatch, opt, 
         failed = False
         try:
             if not skip:
-                call(e)
+                counted(lib, e, call)
         except FplError:
             failed = True
         kind = lib.emu_failed_handle_kind() if lib.emu_fail_handle(0) == 0 else 0
